@@ -4,6 +4,7 @@
 
     python bench.py --gpus N --steps K --warmup W          # our engine
     python bench.py --impl reference --gpus N ...          # unmodified reference (baseline/_ref)
+    python bench.py ... --dump-outputs DIR                 # + what the last timed step computed, as DIR/<name>.npy
 
 One JSON line is printed by rank 0.  `value` is the whole-job steps/sec summed
 over all N GPUs (each rank trains its own 1024-seed batch per step: weak
@@ -249,6 +250,8 @@ def time_trainer(args, rt, tr, nodes, steps, clocks=None):
     ev1.record()
     torch.cuda.synchronize(); rt.barrier()
     ms_dev = ev0.elapsed_time(ev1)
+    if getattr(args, "dump_outputs", None):
+        tr._dump = snapshot_outputs(tr)
     ev2, ev3 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     import graphlearn_b200 as gl
     rt.barrier(); torch.cuda.synchronize()
@@ -276,6 +279,30 @@ def time_trainer(args, rt, tr, nodes, steps, clocks=None):
     return float(t[0]), float(t[1]), final_loss
 
 
+def snapshot_outputs(tr):
+    """What the last device-timed step handed back: its loss, the top layer's logits of the step's seed batch and the
+    updated flat parameter vector (fp32 copies, taken right after the timed region)."""
+    return {"loss": tr.loss_out.detach().float().cpu().clone(),
+            "logits": tr.H[-1].detach().float().cpu().clone(),
+            "params": tr.flat_p.detach().float().cpu().clone()}
+
+
+def write_outputs(out_dir, arrays, limit_bytes=64 << 20):
+    """arrays: name -> fp32 tensor.  Larger outputs are replaced by a fixed, seeded sample of their rows (same rows
+    in every run) so that the dump stays under `limit_bytes`."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    per = limit_bytes // max(1, len(arrays))
+    for name, t in arrays.items():
+        t = t.float()
+        if t.numel() * 4 > per:
+            rows = max(1, per // max(1, 4 * (t.numel() // max(1, t.size(0)))))
+            idx = torch.randperm(t.size(0), generator=torch.Generator().manual_seed(0))[:rows].sort().values
+            t = t[idx]
+        np.save(os.path.join(out_dir, name + ".npy"), t.numpy().astype(np.float32))
+
+
 def run_ours(args):
     import torch
 
@@ -297,6 +324,8 @@ def run_ours(args):
     clocks = ClockSampler(rt.local_rank) if rt.rank == 0 else None
     ms_dev, ms_e2e, final_loss = time_trainer(args, rt, tr, nodes, args.steps, clocks)
     clk = clocks.stop() if clocks else None
+    if args.dump_outputs and rt.rank == 0:
+        write_outputs(args.dump_outputs, tr._dump)
     own, lib, names = count_own_launches(tr)
     # payload bytes of a feature row (the 128-byte aligned stride adds padding that is never read)
     row_bytes = (nodes.float_dim + 2 * ((nodes.float_dim + 31) // 32)) if nodes.feats.local.dtype == torch.uint8 \
@@ -358,7 +387,6 @@ def run_ours(args):
                                          "replica cache of remote feature rows in local HBM (reference: set_local_node_cache_capacity)"),
                        "remote_feature_bytes_per_step_per_gpu": int(remote_bytes),
                        "remote_feature_GBps_per_gpu": round(remote_bytes / (ms_dev / args.steps * 1e-3) / 1e9, 1),
-                       "nvlink_peer_copy_GBps_measured": 770,
                        "seeds": "fresh seed batch every step in both timed regions (device region: resident on the device; "
                                 "e2e region: GSL shuffle(traverse=True) epochs on the host)",
                        "l2_policy": "inputs larger than L2: every step gathers ~%d random feature rows from a %.1f GB table"
@@ -651,8 +679,15 @@ def main():
                     help="gsl = in-memory sources -> gl.Graph -> GSL query -> compiled plan -> engine; raw = shards handed to the trainer")
     ap.add_argument("--no-secondary", action="store_true", help="skip the labelled secondary run (replica cache / other row dtype)")
     ap.add_argument("--small", action="store_true", help="small graph for quick functional runs")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last device-timed step computed (loss, logits of its seed "
+                         "batch, updated parameters) as DIR/<name>.npy (fp32, <= 64 MB in all); inputs are seeded, so two "
+                         "builds can be compared output for output.  Gradients are reduced with fp32 atomics, so runs drift "
+                         "apart with the number of steps: compare short runs (e.g. --steps 20 --warmup 3)")
     args = ap.parse_args()
     args.cfg = CONFIGS[args.config]
+    if args.dump_outputs and (args.impl != "ours" or args.engine != "fast" or "fanouts" not in args.cfg or "heads" in args.cfg):
+        ap.error("--dump-outputs covers the fast GraphSAGE engine (--impl ours --engine fast, configs products_sage2 / sage3)")
     world = int(os.environ.get("WORLD_SIZE", "1"))
     if args.gpus > 1 and world == 1:
         # convenience: re-launch under torchrun

@@ -3,7 +3,7 @@
 // of a 2-hop GSL-style query through the prefetching Dataset.
 //
 // Build:  make -C examples/cpp        (after `python -m graphlearn_b200._build`; links _C.so + libtorch + libpython)
-// Run on a machine with a B200:  ./sample_and_lookup
+// Run on a machine with an H100:  ./sample_and_lookup
 #include <cstdio>
 #include <memory>
 

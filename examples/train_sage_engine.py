@@ -1,4 +1,4 @@
-"""The flagship path: hash-partitioned graph in HBM, fused sm_100a kernels, CUDA-graph step.
+"""The flagship path: hash-partitioned graph in HBM, fused sm_90a kernels, CUDA-graph step.
     torchrun --nproc-per-node 8 --master-addr 127.0.0.1 examples/train_sage_engine.py
 (needs CUDA; on CPU use train_ego_sage.py)."""
 import argparse

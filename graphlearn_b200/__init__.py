@@ -1,4 +1,4 @@
-"""graphlearn_b200 - a B200-native distributed GNN training engine with the
+"""graphlearn_b200 - an H100-native distributed GNN training engine with the
 capabilities and user API of alibaba/graph-learn (``import graphlearn_b200 as gl``).
 
 Public surface mirrors graphlearn/__init__.py:16-40: ``gl.Graph``, ``gl.Dataset``,
@@ -43,7 +43,7 @@ from . import nn  # noqa: E402,F401  (gl.nn, like the reference's `import graphl
 
 class IndexOption(object):
     """KNN index options of the reference (graphlearn/python/c/py_export.cc): ``index_type`` in
-    flat | ivfflat | ivfpq (+ the ``gpu_`` variants); flat = fused tcgen05 scan, ivfflat = k-means lists scanned
+    flat | ivfflat | ivfpq (+ the ``gpu_`` variants); flat = fused wgmma scan, ivfflat = k-means lists scanned
     exactly, ivfpq = the same lists with ``m`` one-byte product-quantiser codes per row, scored by look-up tables and
     re-ranked exactly (ops/knn.py)."""
 

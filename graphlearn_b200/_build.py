@@ -1,7 +1,7 @@
 """In-tree build of the native extension ``graphlearn_b200._C``.
 
-Compiles every ``csrc/*.cu`` / ``*.cpp`` for sm_100a only
-(``-gencode arch=compute_100a,code=sm_100a -lineinfo``) with
+Compiles every ``csrc/*.cu`` / ``*.cpp`` for sm_90a only
+(``-gencode arch=compute_90a,code=sm_90a -lineinfo``) with
 ``torch.utils.cpp_extension`` and leaves the resulting ``_C.so`` inside the
 package directory, so that the snapshot shipped to a GPU box already contains
 the binary (a JIT cache under ~/.cache would not travel).
@@ -25,7 +25,7 @@ _STAMP = os.path.join(_PKG_DIR, "_C.stamp")
 
 CUDA_FLAGS = [
     "-O3",
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo",
     "--expt-relaxed-constexpr",
     "-Xptxas", "-v",
@@ -63,7 +63,7 @@ def build(verbose: bool = False, force: bool = False) -> str:
     if is_fresh() and not force:
         return _SO_PATH
     # torch's own arch list must not add more -gencode flags
-    os.environ["TORCH_CUDA_ARCH_LIST"] = "10.0a"
+    os.environ["TORCH_CUDA_ARCH_LIST"] = "9.0a"
     os.environ.setdefault("MAX_JOBS", str(max(1, (os.cpu_count() or 4) - 1)))
     from torch.utils import cpp_extension
 

@@ -61,7 +61,7 @@ class Config:
     server_id: int = 0
     server_count: int = 1
     server_hosts: str = ""
-    # --- B200 engine specific
+    # --- GPU engine specific
     feature_dtype: str = "fp32"          # fp32 | bf16 | fp8 (e4m3, bf16 scale per 32 elements)   storage of float tables in HBM
     loader_threads: int = 0           # 0 = auto: all cores divided by the number of ranks on the box
     use_peer_kernels: bool = True        # False -> torch.distributed (NCCL/gloo) baseline path
@@ -186,7 +186,7 @@ def set_default_attribute(int_value=None, float_value=None, string_value=None):
 
 def enable_actor():
     """The reference switches to its hiactor runtime (graphlearn/src/service/server.cc:52-60): per-core sharded stores
-    + (data-size aware) tape dispatch.  On B200 the SM grid is the sharded executor; what the flag turns on is the
+    + (data-size aware) tape dispatch.  On the GPU the SM grid is the sharded executor; what the flag turns on is the
     balanced batch dispatch of engine/dispatch.py: multi-rank GSL root traversals pool their seed batches every epoch
     and hand every rank the same number of batches with balanced first-hop work."""
     _CFG.actor_enabled = True

@@ -114,7 +114,7 @@ void save_embeddings(const std::string&, const at::Tensor&, const at::Tensor&, b
 }  // namespace glb
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
-  m.doc() = "graphlearn_b200 native runtime: sm_100a kernels + host loader";
+  m.doc() = "graphlearn_b200 native runtime: sm_90a kernels + host loader";
   // ---- public C++ API (include/glb/api.h), exported 1:1 so the test-suite can hold it against the Python path
   {
     namespace A = glb::api;

@@ -208,7 +208,7 @@ adam_flat_kernel(float* __restrict__ w, const float* __restrict__ g, float* __re
 // Adam fused with everything the next step needs from the parameters (engine/fast_sage.py):
 //   * the gradient (and the scratch accumulators behind it) is zeroed in the same pass - no memset per step
 //   * every weight matrix is re-emitted as the bf16 SWIZZLE_128B K-major image the fused forward kernel feeds
-//     to tcgen05.mma (and, for layers >= 2, the image of W^T used by dA = dZ . W) - no pack kernels per step
+//     to wgmma (and, for layers >= 2, the image of W^T used by dA = dZ . W) - no pack kernels per step
 //   * the loss accumulated by the fused CE epilogue is moved to `loss_out` before it is cleared
 // One thread owns 8 consecutive parameters (parameter starts are 8-aligned in the flat buffer).
 // ---------------------------------------------------------------------------

@@ -1,4 +1,4 @@
-// Common device-side utilities for the graphlearn_b200 sm_100a kernels.
+// Common device-side utilities for the graphlearn_b200 sm_90a kernels.
 //
 // * PeerTable   — by-value table of per-rank base pointers (NVLink P2P / IPC
 //                 mapped).  Every sharded array (CSR indptr/indices, feature

@@ -8,7 +8,7 @@
 // and because sum_j coef_j = 1 the projection commutes with the aggregation:
 //     ret_h = W_n,h ( sum_j coef_j n_j ) + b_n,h .
 // So the layer is: THIS kernel (rows pulled straight from the local / peer-mapped feature shards, one online-softmax
-// pass, H attention-weighted sums of the RAW rows -> bf16 A [M, H * kp]) followed by ONE tcgen05 GEMM with the
+// pass, H attention-weighted sums of the RAW rows -> bf16 A [M, H * kp]) followed by ONE wgmma GEMM with the
 // concatenated W_n,h (K = H * kp) on the persistent kernel of sage_fused.cu - the [M*k, H*D] projected neighbour
 // tensor of the reference never exists.
 //

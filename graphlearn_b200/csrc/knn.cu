@@ -1,15 +1,15 @@
-// K10: brute-force KNN as ONE kernel per 128-query tile - score GEMM on tcgen05 with a fused running top-k,
+// K10: brute-force KNN as ONE kernel per 128-query tile - score GEMM on wgmma with a fused running top-k,
 // the [B, N] score matrix is never materialised.
 //
 //   scores[q, x] = <Q[q], X[x]>            (inner product)      or      2 <Q[q], X[x]> - |X[x]|^2     (L2; larger = closer)
 //
 // Every CTA (one per SM) owns a contiguous range of database rows and walks it in slabs of 128 rows:
-//   warps 5..12  producers : database rows (fp32 or bf16, optionally through a row-index list = an IVF inverted
+//   warps 4..11  producers : database rows (fp32 or bf16, optionally through a row-index list = an IVF inverted
 //                            list) -> bf16 -> K-major SWIZZLE_128B operand tile in shared memory (double buffered)
-//   warp  4      MMA       : D[128 queries x 128 rows] = Q . X_slab^T, one elected lane issues tcgen05.mma into one of
-//                            two TMEM accumulators
-//   warps 0..3   top-k     : one thread per query drains its 128 scores (tcgen05.ld) and keeps the k best (value, row)
-//                            in shared memory behind a register-held admission threshold
+//   warps 0..3   MMA+top-k : one warpgroup computes D[128 queries x 32 rows] = Q . X^T slice by slice with wgmma
+//                            (two M=64 halves, fp32 accumulators in registers), parks the slice in shared memory, and
+//                            then one thread per query scans its 32 scores and keeps the k best (value, row) in shared
+//                            memory behind a register-held admission threshold
 // The per-CTA lists are merged by knn_merge_kernel (one warp per query), which also reads the partial lists of PEER GPUs
 // straight from their HBM (the reference broadcasts the query to every server and merges with a k-heap over gRPC:
 // graphlearn/src/contrib/knn/knn_request.cc:96-111,167-202; index types: index_factory.cc:28-50).
@@ -19,14 +19,16 @@
 #include <cfloat>
 #include <cstring>
 #include "host_utils.h"
-#include "umma.cuh"
+#include "gmma.cuh"
 
 namespace glb {
 
-constexpr int kKnnQ = 128;                 // queries per tile (UMMA M)
-constexpr int kKnnSlab = 128;              // database rows per slab (UMMA N)
-constexpr int kKnnTopWarps = 4, kKnnMmaWarp = 4, kKnnProdWarp0 = 5, kKnnProdWarps = 8;
-constexpr int kKnnThreads = (kKnnProdWarp0 + kKnnProdWarps) * 32;   // 416
+constexpr int kKnnQ = 128;                 // queries per tile (two wgmma M = 64 halves)
+constexpr int kKnnSlab = 128;              // database rows per slab
+constexpr int kKnnSlice = 32;              // database rows per MMA slice (wgmma N)
+constexpr int kKnnScoreLd = kKnnSlice + 1; // row pitch of the staged score slice (conflict-free per-query reads)
+constexpr int kKnnTopWarps = 4, kKnnProdWarp0 = 4, kKnnProdWarps = 8;
+constexpr int kKnnThreads = (kKnnProdWarp0 + kKnnProdWarps) * 32;   // 384
 constexpr int kKnnMaxK = 64;
 
 struct KnnParams {
@@ -39,24 +41,23 @@ struct KnnParams {
   float* out_s;                                      // [grid, 128, k] partial scores
   int64_t* out_i;                                    // [grid, 128, k] partial row indices (into x / row_list space)
   int64_t rows_per_cta;
+  int n_xbuf;                                        // database slab buffers: 2 (double buffered) or 1 when two do not fit
 };
 
 __global__ void __launch_bounds__(kKnnThreads, 1) knn_flat_kernel(const __grid_constant__ KnnParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024u - (umma::smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint8_t* smem = smem_raw + ((1024u - (gmma::smem_u32(smem_raw) & 1023u)) & 1023u);
   const int nkb = p.dpad >> 6;
   const uint32_t tile_bytes = (uint32_t)nkb * (128 * 128);
   uint8_t* sQ = smem;
-  uint8_t* sX = sQ + tile_bytes;                                   // [2] slabs
-  float* sNorm = reinterpret_cast<float*>(sX + 2 * tile_bytes);    // [2][128]
-  float* topv = sNorm + 2 * kKnnSlab;                              // [k][128]
+  uint8_t* sX = sQ + tile_bytes;                                   // [n_xbuf] slabs
+  float* sNorm = reinterpret_cast<float*>(sX + (size_t)p.n_xbuf * tile_bytes);   // [n_xbuf][128]
+  float* sScore = sNorm + p.n_xbuf * kKnnSlab;                     // [128][kKnnScoreLd] one score slice
+  float* topv = sScore + kKnnQ * kKnnScoreLd;                      // [k][128]
   int* topi = reinterpret_cast<int*>(topv + (size_t)p.k * kKnnQ);  // [k][128]  (slab-relative global index as int)
   uint64_t* bars = reinterpret_cast<uint64_t*>(topi + (size_t)p.k * kKnnQ);
   uint64_t* x_full = bars;          // [2] producers -> MMA
-  uint64_t* x_free = bars + 2;      // [2] MMA -> producers
-  uint64_t* t_full = bars + 4;      // [2] MMA -> top-k
-  uint64_t* t_free = bars + 6;      // [2] top-k -> MMA
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 8);
+  uint64_t* x_free = bars + 2;      // [2] MMA / top-k -> producers (operand tile and norm slice consumed)
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int64_t r_begin = (int64_t)blockIdx.x * p.rows_per_cta;
@@ -65,14 +66,11 @@ __global__ void __launch_bounds__(kKnnThreads, 1) knn_flat_kernel(const __grid_c
 
   if (tid == 0) {
     for (int i = 0; i < 2; ++i) {
-      umma::mbar_init(x_full + i, kKnnProdWarps);
-      umma::mbar_init(x_free + i, 1);
-      umma::mbar_init(t_full + i, 1);
-      umma::mbar_init(t_free + i, kKnnTopWarps);
+      gmma::mbar_init(x_full + i, kKnnProdWarps);
+      gmma::mbar_init(x_free + i, kKnnTopWarps);
     }
-    umma::fence_barrier_init();
+    gmma::fence_barrier_init();
   }
-  if (warp == kKnnMmaWarp) { umma::tmem_alloc(tmem_slot, 256); umma::tmem_relinquish(); }
   // query tile -> SW128 K-major (all threads), top-k lists cleared
   {
     const int chunks_row = p.dpad >> 3;
@@ -80,38 +78,55 @@ __global__ void __launch_bounds__(kKnnThreads, 1) knn_flat_kernel(const __grid_c
       const int r = i / chunks_row, c = i - r * chunks_row;
       const uint4 v = *reinterpret_cast<const uint4*>(p.q + (size_t)r * p.dpad + c * 8);
       const int kcol = c * 8;
-      *reinterpret_cast<uint4*>(sQ + (size_t)(kcol >> 6) * (128 * 128) + umma::sw128_offset((uint32_t)r, (uint32_t)(kcol & 63))) = v;
+      *reinterpret_cast<uint4*>(sQ + (size_t)(kcol >> 6) * (128 * 128) + gmma::sw128_offset((uint32_t)r, (uint32_t)(kcol & 63))) = v;
     }
     for (int i = tid; i < p.k * kKnnQ; i += kKnnThreads) { topv[i] = -FLT_MAX; topi[i] = -1; }
   }
-  umma::fence_proxy_async_smem();
-  umma::tc_fence_before();
+  gmma::fence_proxy_async_smem();
   __syncthreads();
-  umma::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp < kKnnTopWarps) {
-    // ------------------------------------------------------------------ running top-k (thread = query)
+    // ------------------------------------------------------------------ score MMA + running top-k (thread = query)
     const int q = warp * 32 + lane;
     float thr = -FLT_MAX;                                   // smallest kept score (admission threshold)
     int thr_pos = 0;
+    const uint32_t q_base = gmma::smem_u32(sQ);
     for (int s = 0; s < n_slabs; ++s) {
-      const int b = s & 1;
-      umma::mbar_wait(t_full + b, (uint32_t)((s >> 1) & 1));
-      umma::tc_fence_after();
+      const int b = s % p.n_xbuf;
+      gmma::mbar_wait(x_full + b, (uint32_t)((s / p.n_xbuf) & 1));
       const int64_t base = r_begin + (int64_t)s * kKnnSlab;
       const int valid = (int)min((int64_t)kKnnSlab, r_end - base);
-      const uint32_t taddr = tmem_base + (uint32_t)(b * kKnnSlab) + ((uint32_t)(warp * 32) << 16);
-      for (int c0 = 0; c0 < kKnnSlab; c0 += 32) {
-        if (c0 >= valid) break;
-        uint32_t v[32];
-        umma::tmem_ld32(taddr + (uint32_t)c0, v);
-        umma::tmem_ld_wait();
-        if (q < p.B) {
+      const uint32_t x_base = gmma::smem_u32(sX + (size_t)b * tile_bytes);
+      for (int c0 = 0; c0 < valid; c0 += kKnnSlice) {
 #pragma unroll
-          for (int i = 0; i < 32; ++i) {
+        for (int mh = 0; mh < 2; ++mh) {
+          float d[16];
+          gmma::wgmma_fence();
+          for (int kb = 0; kb < nkb; ++kb) {
+            const uint32_t a_kb = q_base + (uint32_t)kb * (128 * 128) + (uint32_t)mh * (64 * 128);
+            const uint32_t b_kb = x_base + (uint32_t)kb * (128 * 128) + (uint32_t)c0 * 128;
+#pragma unroll
+            for (int k4 = 0; k4 < 4; ++k4)
+              gmma::mma_m64n32_bf16<0, 0>(d, gmma::make_desc_sw128(a_kb + k4 * 32), gmma::make_desc_sw128(b_kb + k4 * 32), (kb | k4) ? 1u : 0u);
+          }
+          gmma::wgmma_commit();
+          gmma::wgmma_wait<0>();
+          gmma::fence_regs(d);
+          const int r = mh * 64 + warp * 16 + (lane >> 2);
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            const int c = 8 * j + 2 * (lane & 3);
+            sScore[r * kKnnScoreLd + c] = d[4 * j];
+            sScore[r * kKnnScoreLd + c + 1] = d[4 * j + 1];
+            sScore[(r + 8) * kKnnScoreLd + c] = d[4 * j + 2];
+            sScore[(r + 8) * kKnnScoreLd + c + 1] = d[4 * j + 3];
+          }
+        }
+        asm volatile("bar.sync 1, %0;" ::"n"(kKnnTopWarps * 32) : "memory");     // the slice's scores are staged
+        if (q < p.B) {
+          for (int i = 0; i < kKnnSlice; ++i) {
             if (c0 + i < valid) {
-              float sc = __uint_as_float(v[i]);
+              float sc = sScore[q * kKnnScoreLd + i];
               if (p.x_norm) sc = 2.f * sc - sNorm[b * kKnnSlab + c0 + i];
               if (sc > thr) {
                 topv[thr_pos * kKnnQ + q] = sc;
@@ -125,10 +140,10 @@ __global__ void __launch_bounds__(kKnnThreads, 1) knn_flat_kernel(const __grid_c
             }
           }
         }
+        asm volatile("bar.sync 1, %0;" ::"n"(kKnnTopWarps * 32) : "memory");     // the staging slice may be overwritten
       }
-      umma::tc_fence_before();
       __syncwarp();
-      if (lane == 0) umma::mbar_arrive(t_free + b);
+      if (lane == 0) gmma::mbar_arrive(x_free + b);
     }
     // publish this CTA's list
     if (q < p.B) {
@@ -140,37 +155,14 @@ __global__ void __launch_bounds__(kKnnThreads, 1) knn_flat_kernel(const __grid_c
         oi[j] = li < 0 ? -1 : (p.row_list ? p.row_list[r_begin + li] : r_begin + li);
       }
     }
-  } else if (warp == kKnnMmaWarp) {
-    // ------------------------------------------------------------------ MMA issuer
-    const uint32_t idesc = umma::make_idesc_bf16(kKnnQ, kKnnSlab);
-    for (int s = 0; s < n_slabs; ++s) {
-      const int b = s & 1;
-      umma::mbar_wait(x_full + b, (uint32_t)((s >> 1) & 1));
-      umma::mbar_wait(t_free + b, (uint32_t)(((s >> 1) & 1) ^ 1));
-      umma::tc_fence_after();
-      if (lane == 0) {
-        const uint32_t d = tmem_base + (uint32_t)(b * kKnnSlab);
-        for (int kb = 0; kb < nkb; ++kb) {
-          const uint32_t a_base = umma::smem_u32(sQ + (size_t)kb * (128 * 128));
-          const uint32_t b_base = umma::smem_u32(sX + (size_t)b * tile_bytes + (size_t)kb * (128 * 128));
-#pragma unroll
-          for (int k4 = 0; k4 < 4; ++k4)
-            umma::mma_bf16_ss(d, umma::make_desc_sw128(a_base + k4 * 32), umma::make_desc_sw128(b_base + k4 * 32), idesc, (kb | k4) ? 1u : 0u);
-        }
-        umma::mma_commit(x_free + b);
-        umma::mma_commit(t_full + b);
-      }
-      __syncwarp();
-    }
   } else {
     // ------------------------------------------------------------------ producers: database slab -> bf16 SW128 tile
     const int pt = tid - kKnnProdWarp0 * 32;                 // 0..255
     const int chunks_row = p.dpad >> 3;                      // 16-byte bf16 chunks per row
     const int per_slab = kKnnSlab * chunks_row;
     for (int s = 0; s < n_slabs; ++s) {
-      const int b = s & 1;
-      umma::mbar_wait(x_free + b, (uint32_t)(((s >> 1) & 1) ^ 1));     // the MMA has consumed the operand tile
-      umma::mbar_wait(t_free + b, (uint32_t)(((s >> 1) & 1) ^ 1));     // the top-k warps have consumed the norm slice
+      const int b = s % p.n_xbuf;
+      gmma::mbar_wait(x_free + b, (uint32_t)(((s / p.n_xbuf) & 1) ^ 1));     // MMA and top-k are done with the tile and norm slice
       const int64_t base = r_begin + (int64_t)s * kKnnSlab;
       uint8_t* dst = sX + (size_t)b * tile_bytes;
       // batches of 8 chunks per thread: all loads of a batch are issued before the first store (one DRAM round trip per
@@ -210,7 +202,7 @@ __global__ void __launch_bounds__(kKnnThreads, 1) knn_flat_kernel(const __grid_c
           if (i < per_slab) {
             const int r = i / chunks_row, c = i - r * chunks_row;
             const int kcol = c * 8;
-            *reinterpret_cast<uint4*>(dst + (size_t)(kcol >> 6) * (128 * 128) + umma::sw128_offset((uint32_t)r, (uint32_t)(kcol & 63))) = vals[u];
+            *reinterpret_cast<uint4*>(dst + (size_t)(kcol >> 6) * (128 * 128) + gmma::sw128_offset((uint32_t)r, (uint32_t)(kcol & 63))) = vals[u];
           }
         }
       }
@@ -218,14 +210,11 @@ __global__ void __launch_bounds__(kKnnThreads, 1) knn_flat_kernel(const __grid_c
         const int64_t li = base + pt;
         sNorm[b * kKnnSlab + pt] = li < r_end ? __ldg(p.x_norm + (p.row_list ? __ldg(p.row_list + li) : li)) : 0.f;
       }
-      umma::fence_proxy_async_smem();
+      gmma::fence_proxy_async_smem();
       __syncwarp();
-      if (lane == 0) umma::mbar_arrive(x_full + b);
+      if (lane == 0) gmma::mbar_arrive(x_full + b);
     }
   }
-  umma::tc_fence_before();
-  __syncthreads();
-  if (warp == kKnnMmaWarp) umma::tmem_dealloc(tmem_base, 256);
 }
 
 // k-way merge: one warp per query selects the k best of all candidate lists - the partial lists of this GPU's CTAs or
@@ -433,7 +422,11 @@ std::vector<at::Tensor> knn_flat_topk(const at::Tensor& x, int64_t dim, const c1
   auto part_i = at::empty({grid, kKnnQ, k}, oi);
   p.out_s = part_s.data_ptr<float>(); p.out_i = part_i.data_ptr<int64_t>();
   const size_t tile = (size_t)(p.dpad / 64) * 128 * 128;
-  const size_t smem = 1024 + 3 * tile + 2 * kKnnSlab * 4 + (size_t)k * kKnnQ * 8 + 9 * 8 + 16;
+  auto smem_for = [&](int nbuf) {
+    return 1024 + (size_t)(1 + nbuf) * tile + (size_t)nbuf * kKnnSlab * 4 + (size_t)kKnnQ * kKnnScoreLd * 4 + (size_t)k * kKnnQ * 8 + 4 * 8;
+  };
+  p.n_xbuf = smem_for(2) <= 232448 ? 2 : 1;                  // wide queries / large k: one slab buffer, no load-MMA overlap
+  const size_t smem = smem_for(p.n_xbuf);
   TORCH_CHECK(smem <= 232448, "query width too large for the fused KNN tile");
   static size_t attr = 0;
   if (smem > attr) { C10_CUDA_CHECK(cudaFuncSetAttribute(knn_flat_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); attr = smem; }

@@ -1,13 +1,13 @@
-// Backward of the fused GraphSAGE layer on the 5th-gen tensor cores (replaces the library GEMMs of round 1).
+// Backward of the fused GraphSAGE layer on the Hopper tensor cores (warpgroup MMA, wgmma).
 //
 //   dW_l [n_out, K_total] += dZ_l^T . A_l          (reduction over the 10^4..10^5 destination rows of the layer)
 //
-// Both operands are row-major with the REDUCTION index outermost, i.e. exactly the "MN-major" operand form
-// of tcgen05.mma: a [64 rows x 64 cols] bf16 slab is one SWIZZLE_128B atom column (K = row index), so the
+// Both operands are row-major with the REDUCTION index outermost, i.e. exactly the "MN-major" (transposed) operand
+// form of wgmma: a [64 rows x 64 cols] bf16 slab is one SWIZZLE_128B atom column (K = row index), so the
 // tiles are staged with plain coalesced 16-byte loads + swizzled 16-byte shared stores - no transpose.
 //
-// Split-K over the whole chip: CTA (block, split) owns a [128 x <=256] block of dW and a contiguous range
-// of rows; it accumulates in TMEM (fp32) over its rows and adds the partial block to the flat gradient
+// Split-K over the whole chip: CTA (block, split) owns a [128 x <=128] block of dW and a contiguous range
+// of rows; it accumulates in registers (fp32) over its rows and adds the partial block to the flat gradient
 // buffer with vectorised red.global.add (the gradient buffer is zeroed once per step).
 //
 // The dZ operand is usually not read but COMPUTED on the fly (fused "backward through ReLU + mean
@@ -16,9 +16,11 @@
 // so dZ of the big hop segments never exists in HBM for 2-layer models; the bias gradient (column sums of
 // dZ) falls out of the same registers.  Deeper models can ask for dZ to be written (needed by dA = dZ.W).
 //
-// warps 0..15 : producers (loads -> ReLU-grad math -> swizzled st.shared), later the epilogue (tcgen05.ld -> red);
-//               warp 0 also owns TMEM and issues the MMAs of a stage once all 16 warps have filled it
-//               (3-stage mbarrier ring, operands of stage st+1 already in flight in registers)
+// warps 0..15 : producers (loads -> ReLU-grad math -> swizzled st.shared) and, as four warpgroups, the MMA issuers:
+//               warpgroup g owns the [64 x 64] quadrant (rows 64 (g & 1), columns 64 (g >> 1)) of the CTA's dW block
+//               and issues its MMAs of a stage once all 16 warps have filled it (3-stage mbarrier ring, operands of
+//               stage st+1 already in flight in registers; a stage is released once wgmma.wait_group reports its
+//               MMAs complete); the epilogue adds the register accumulators with red.global
 //
 // Reference semantics: plain autograd of EgoSAGEConv (graphlearn/python/nn/tf/layers/ego_sage_conv.py:71-106).
 #include <torch/extension.h>
@@ -26,7 +28,7 @@
 #include <c10/cuda/CUDAGuard.h>
 #include <cstring>
 #include "host_utils.h"
-#include "umma.cuh"
+#include "gmma.cuh"
 
 namespace glb {
 
@@ -37,7 +39,8 @@ constexpr int kDwThreads = kDwProdThreads;            // warp 0 doubles as the M
 constexpr int kDwStages = 3;
 constexpr int kDwRows = 64;                           // reduction rows per stage (4 MMA K-steps)
 constexpr int kDwZBytes = kDwRows * 128 * 2;          // dZ slab  [64 rows x 128 cols] bf16 = 16 KB
-constexpr int kDwBBytes = kDwRows * 256 * 2;          // A slab   [64 rows x 256 cols] bf16 = 32 KB
+constexpr int kDwCols = 128;                          // dW columns per CTA (the register accumulators of 4 warpgroups)
+constexpr int kDwBBytes = kDwRows * kDwCols * 2;      // A slab   [64 rows x 128 cols] bf16 = 16 KB
 constexpr int kDwStageBytes = kDwZBytes + kDwBBytes;
 constexpr int kDwMaxSegs = 4;
 
@@ -66,8 +69,8 @@ struct DwParams {
 
 __device__ __forceinline__ uint4 ldg16(const void* p) { return *reinterpret_cast<const uint4*>(p); }
 
-__device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float c, float d) {
-  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
+__device__ __forceinline__ void red_add_v2(float* addr, float a, float b) {
+  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(a), "f"(b) : "memory");
 }
 
 // byte offset of the 16-byte chunk (row r in [0,64), 8-column chunk c) inside an MN-major SW128 slab whose
@@ -78,14 +81,12 @@ __device__ __forceinline__ uint32_t mn_off(int r, int c) {
 
 __global__ void __launch_bounds__(kDwThreads, 1) sage_bwd_dw_kernel(const __grid_constant__ DwParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024u - (umma::smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint8_t* smem = smem_raw + ((1024u - (gmma::smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* stages = smem;
   float* colsum = reinterpret_cast<float*>(stages + kDwStages * kDwStageBytes);   // [128]
   uint64_t* bars = reinterpret_cast<uint64_t*>(colsum + 128);
   uint64_t* bar_full = bars;                    // [kDwStages] producers -> MMA
   uint64_t* bar_empty = bars + kDwStages;       // [kDwStages] MMA -> producers
-  uint64_t* bar_done = bars + 2 * kDwStages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * kDwStages + 1);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int blk = blockIdx.x % (p.m_blocks * p.n_blocks);
@@ -94,28 +95,28 @@ __global__ void __launch_bounds__(kDwThreads, 1) sage_bwd_dw_kernel(const __grid
   const int r_begin = split * p.rows_per_split;
   const int r_end = min(p.rows, r_begin + p.rows_per_split);
   const int n_steps = (r_end - r_begin + kDwRows - 1) / kDwRows;
-  const int ncols_blk = min(256, p.n_cols - nb * 256);          // multiple of 16
+  const int ncols_blk = min(kDwCols, p.n_cols - nb * kDwCols);  // multiple of 16
 
   if (tid == 0) {
-    for (int i = 0; i < kDwStages; ++i) { umma::mbar_init(bar_full + i, kDwProdWarps); umma::mbar_init(bar_empty + i, 1); }
-    umma::mbar_init(bar_done, 1);
-    umma::fence_barrier_init();
+    for (int i = 0; i < kDwStages; ++i) { gmma::mbar_init(bar_full + i, kDwProdWarps); gmma::mbar_init(bar_empty + i, kDwProdWarps); }
+    gmma::fence_barrier_init();
   }
   if (tid < 128) colsum[tid] = 0.f;
-  if (warp == 0) { umma::tmem_alloc(tmem_slot, 256); umma::tmem_relinquish(); }
-  umma::tc_fence_before();
   __syncthreads();
-  umma::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  const uint32_t idesc = umma::make_idesc_bf16_major(128, ncols_blk, 1, 1);
+  const int wg = warp >> 2, wq = warp & 3;
+  const int mh = wg & 1, nh = wg >> 1;            // this warpgroup's quadrant of the [128 x 128] block
+  const bool wg_active = nh * 64 < ncols_blk;     // warp-uniform: a narrow block leaves the right half idle
+  float acc[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) acc[i] = 0.f;
   {
     // ------------------------------------------------------------------ producers
     const int pt = tid;                              // 0..511
     const int zc = pt & 15, zr = pt >> 4;            // dZ slab: 16 chunks per row, rows zr and zr + 32
-    const int bc = pt & 31, br = pt >> 5;            // A slab : 32 chunks per row, rows br + 16 i
+    const int bc = pt & 15, br = pt >> 4;            // A slab : 16 chunks per row, rows br + 32 i
     const int zcol = mb * 128 + zc * 8;              // first dZ column of this thread's chunk
-    const int bcol = nb * 256 + bc * 8;
+    const int bcol = nb * kDwCols + bc * 8;
     const bool zcol_ok = zcol < p.dz_cols;
     const bool bcol_ok = bcol < p.n_cols;
     const bool want_out = p.dz_out != nullptr && nb == 0;
@@ -125,12 +126,12 @@ __global__ void __launch_bounds__(kDwThreads, 1) sage_bwd_dw_kernel(const __grid
     const uint4 zero4 = make_uint4(0u, 0u, 0u, 0u);
     // register-staged operands of one 64-row stage; two sets are alive so that the loads of stage st+1 are in
     // flight while stage st is converted and stored (the kernel is bound by bytes in flight, not by math)
-    struct StageRegs { uint4 bv[4], hv[2], sv[2], nv[2]; float nscale[2]; };
+    struct StageRegs { uint4 bv[2], hv[2], sv[2], nv[2]; float nscale[2]; };
     auto issue = [&](int st, StageRegs& g) {
       const int rbase = r_begin + st * kDwRows;
 #pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int r = rbase + br + 16 * i;
+      for (int i = 0; i < 2; ++i) {
+        const int r = rbase + br + 32 * i;
         g.bv[i] = (r < r_end && bcol_ok) ? ldg16(p.a + (size_t)r * p.ld_a + bcol) : zero4;
       }
 #pragma unroll
@@ -181,31 +182,32 @@ __global__ void __launch_bounds__(kDwThreads, 1) sage_bwd_dw_kernel(const __grid
         const int r = rbase + zr + 32 * i;
         if (want_out && r < r_end && zcol < p.ld_dz_out) *reinterpret_cast<uint4*>(p.dz_out + (size_t)r * p.ld_dz_out + zcol) = zv[i];
       }
-      umma::mbar_wait(bar_empty + s, (uint32_t)(((st / kDwStages) & 1) ^ 1));
+      gmma::mbar_wait(bar_empty + s, (uint32_t)(((st / kDwStages) & 1) ^ 1));
       uint8_t* zs = stages + (size_t)s * kDwStageBytes;
       uint8_t* bs = zs + kDwZBytes;
 #pragma unroll
       for (int i = 0; i < 2; ++i) *reinterpret_cast<uint4*>(zs + mn_off(zr + 32 * i, zc)) = zv[i];
 #pragma unroll
-      for (int i = 0; i < 4; ++i) *reinterpret_cast<uint4*>(bs + mn_off(br + 16 * i, bc)) = g.bv[i];
-      umma::fence_proxy_async_smem();
+      for (int i = 0; i < 2; ++i) *reinterpret_cast<uint4*>(bs + mn_off(br + 32 * i, bc)) = g.bv[i];
+      gmma::fence_proxy_async_smem();
       __syncwarp();
-      if (lane == 0) umma::mbar_arrive(bar_full + s);
-      if (warp == 0) {
-        // MMA issue for this stage (the operands of the next stage are already in flight in this warp's registers)
-        umma::mbar_wait(bar_full + s, (uint32_t)((st / kDwStages) & 1));
-        umma::tc_fence_after();
-        if (lane == 0) {
-          const uint32_t zb = umma::smem_u32(zs);
-          const uint32_t bb = zb + kDwZBytes;
+      if (lane == 0) gmma::mbar_arrive(bar_full + s);
+      // MMA issue for this stage (the operands of the next stage are already in flight in this warp's registers)
+      gmma::mbar_wait(bar_full + s, (uint32_t)((st / kDwStages) & 1));
+      if (wg_active) {
+        const uint32_t zb = gmma::smem_u32(zs) + (uint32_t)mh * 8192u;         // dZ columns 64 mh .. (mn_off's group stride)
+        const uint32_t bb = gmma::smem_u32(bs) + (uint32_t)nh * 8192u;         // A columns 64 nh ..
+        gmma::wgmma_fence();
 #pragma unroll
-          for (int k4 = 0; k4 < 4; ++k4)
-            umma::mma_bf16_ss(tmem_base, umma::make_desc_sw128_mn(zb + k4 * p.kadv, p.lbo, p.sbo),
-                              umma::make_desc_sw128_mn(bb + k4 * p.kadv, p.lbo, p.sbo), idesc, (st | k4) ? 1u : 0u);
-          umma::mma_commit(bar_empty + s);
-          if (st == n_steps - 1) umma::mma_commit(bar_done);
-        }
+        for (int k4 = 0; k4 < 4; ++k4)
+          gmma::mma_m64n64_bf16<1, 1>(acc, gmma::make_desc_sw128_mn(zb + k4 * p.kadv, p.lbo, p.sbo),
+                                       gmma::make_desc_sw128_mn(bb + k4 * p.kadv, p.lbo, p.sbo), 1u);
+        gmma::wgmma_commit();
+        gmma::wgmma_wait<1>();                            // the MMAs of stage st-1 have completed
+      }
+      if (st > 0) {
         __syncwarp();
+        if (lane == 0) gmma::mbar_arrive(bar_empty + (st - 1) % kDwStages);
       }
     };
     StageRegs ra, rb;
@@ -221,13 +223,14 @@ __global__ void __launch_bounds__(kDwThreads, 1) sage_bwd_dw_kernel(const __grid
     // bias gradient = column sums of the computed dZ (only the n-block-0 CTAs of an m-block contribute): the two
     // rows of a warp are folded with a shuffle, every warp parks its 128 sums in the (now idle) stage memory and
     // 128 threads add the 16 rows up - no shared-memory atomics (they were 32-way same-address conflicts)
+    gmma::wgmma_wait<0>();
+    gmma::fence_regs(acc);
     const bool do_bias = p.dbias && !p.dz && nb == 0 && n_steps > 0;
     if (do_bias) {
 #pragma unroll
       for (int i = 0; i < 8; ++i) cs[i] += __shfl_xor_sync(0xffffffffu, cs[i], 16);
-      // all MMAs have been issued and committed by the time the last stage was filled; wait for them before the
-      // stage memory is reused
-      umma::mbar_wait(bar_done, 0);
+      // every warpgroup's MMAs must have completed before the stage memory is reused
+      __syncthreads();
       float* wsum = reinterpret_cast<float*>(stages) + warp * 128;
       if (lane < 16) {
         *reinterpret_cast<float4*>(wsum + zc * 8) = make_float4(cs[0], cs[1], cs[2], cs[3]);
@@ -242,32 +245,21 @@ __global__ void __launch_bounds__(kDwThreads, 1) sage_bwd_dw_kernel(const __grid
     for (int w = 0; w < kDwProdWarps; ++w) v += reinterpret_cast<const float*>(stages)[w * 128 + tid];
     atomicAdd(p.dbias + mb * 128 + tid, v);
   }
-  // ------------------------------------------------------------------ epilogue: TMEM -> red.global.add into dW
-  if (n_steps > 0) {
-    umma::mbar_wait(bar_done, 0);
-    umma::tc_fence_after();
-    const int q = warp & 3;                       // TMEM lane quarter
-    const int cq = warp >> 2;                     // column quarter (64 columns each)
-    const int m = mb * 128 + q * 32 + lane;
-    const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16);
-    for (int c0 = cq * 64; c0 < cq * 64 + 64; c0 += 32) {
-      if (c0 >= ncols_blk) break;                 // warp-uniform
-      uint32_t v[32];
-      umma::tmem_ld32(taddr + (uint32_t)c0, v);
-      umma::tmem_ld_wait();
-      if (m < p.n_out && !p.skip_red) {
-        float* dst = p.dw + (size_t)m * p.ld_dw + nb * 256 + c0;
+  // ------------------------------------------------------------------ epilogue: registers -> red.global.add into dW
+  if (n_steps > 0 && wg_active && !p.skip_red) {
+    const int r0 = mh * 64 + wq * 16 + (lane >> 2);
 #pragma unroll
-        for (int i = 0; i < 8; ++i)
-          if (c0 + 4 * i < ncols_blk)
-            red_add_v4(dst + 4 * i, __uint_as_float(v[4 * i]), __uint_as_float(v[4 * i + 1]), __uint_as_float(v[4 * i + 2]),
-                       __uint_as_float(v[4 * i + 3]));
+    for (int j = 0; j < 8; ++j) {
+      const int c = nh * 64 + 8 * j + 2 * (lane & 3);
+      if (c < ncols_blk) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int m = mb * 128 + r0 + 8 * h;
+          if (m < p.n_out) red_add_v2(p.dw + (size_t)m * p.ld_dw + nb * kDwCols + c, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+        }
       }
     }
   }
-  umma::tc_fence_before();
-  __syncthreads();
-  if (warp == 0) umma::tmem_dealloc(tmem_base, 256);
 }
 
 // fp32 master weight [n_out, k_total] -> bf16 K-major SW128 images of W^T for the dA = dZ . W GEMM:
@@ -377,7 +369,7 @@ void sage_bwd_dw(const c10::optional<at::Tensor>& dz, const c10::optional<at::Te
   }
   if (p.rows == 0) return;
   p.m_blocks = (p.n_out + 127) / 128;
-  p.n_blocks = (p.n_cols + 255) / 256;
+  p.n_blocks = (p.n_cols + kDwCols - 1) / kDwCols;
   const int blocks = p.m_blocks * p.n_blocks;
   const int sms = sm_count();
   const int max_splits = std::max(1, sms / blocks);
@@ -388,7 +380,7 @@ void sage_bwd_dw(const c10::optional<at::Tensor>& dz, const c10::optional<at::Te
   p.lbo = 8192; p.sbo = 1024; p.kadv = 2048;
   if (desc_override.size() == 4) p.skip_red = (int)desc_override[3];
   if (desc_override.size() >= 3) { p.lbo = (uint32_t)desc_override[0]; p.sbo = (uint32_t)desc_override[1]; p.kadv = (uint32_t)desc_override[2]; }
-  const size_t smem = 1024 + (size_t)kDwStages * kDwStageBytes + 512 + (2 * kDwStages + 2) * 8;
+  const size_t smem = 1024 + (size_t)kDwStages * kDwStageBytes + 512 + 2 * kDwStages * 8;
   static bool attr_done = false;
   if (!attr_done) {
     C10_CUDA_CHECK(cudaFuncSetAttribute(sage_bwd_dw_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

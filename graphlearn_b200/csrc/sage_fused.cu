@@ -13,18 +13,19 @@
 //                             NVLink, or the local replica cache) in a private SMEM scratch - the ids of the
 //                             NEXT item are prefetched while the current rows are in flight -, pulls the self
 //                             row and the k neighbour rows with batches of 16-byte loads, reduces in fp32
-//                             registers and writes the bf16 A tile in the UMMA K-major SWIZZLE_128B layout
+//                             registers and writes the bf16 A tile in the wgmma K-major SWIZZLE_128B layout
 //                             (and row-major to global for the backward pass); items are dealt round-robin
 //                             ACROSS tile boundaries so no warp idles; the A tile is double buffered; rows may be
 //                             fp32, bf16 or block-scaled fp8 (dequantised while accumulating)
-//   MMA warp (1)              W image fetched ONCE per CTA by the TMA engine (cp.async.bulk); one
-//                             elected thread issues tcgen05.mma (M=64, N<=256, K=16) into one of two
-//                             TMEM accumulators; tcgen05.commit frees the A tile and publishes the
-//                             accumulator through mbarriers
-//   epilogue warps (EW, default 4)  tcgen05.ld -> bias -> ReLU -> bf16/fp32 store of tile t while the gather
-//                             warps are already loading tile t+1; for the top layer a second, coalesced
-//                             phase (one warp per row, one lane per class) computes the softmax
-//                             cross-entropy loss, dlogits and the bias gradient (fused CE)
+//   W warp (1)                W image fetched ONCE per CTA by the TMA engine (cp.async.bulk)
+//   MMA + epilogue warps (EW, default 4 = one warpgroup)  per 32-column slice of the output: wgmma
+//                             (M=64, N=32, K=16) over the whole K with the fp32 accumulator in registers,
+//                             then bias -> ReLU -> bf16/fp32 store, while the gather warps are already
+//                             filling the other A buffer with tile t+1; an mbarrier arrival after the last
+//                             slice's MMAs frees the A tile.  Two warpgroups (EW = 8) take alternate slices.
+//                             For the top layer a second, coalesced phase (one warp per row, one lane per
+//                             class) computes the softmax cross-entropy loss, dlogits and the bias gradient
+//                             (fused CE)
 //
 // The rows never round-trip through HBM ("agg(X).W" instead of materialising [B*k, D]).
 //
@@ -37,15 +38,15 @@
 #include <cfloat>
 #include <cstring>
 #include "host_utils.h"
-#include "umma.cuh"
+#include "gmma.cuh"
 #include "gather_common.cuh"
 
 namespace glb {
 
-constexpr int kTileM = 64;                         // destination rows per tile = UMMA M (two A tiles fit next to the W image)
+constexpr int kTileM = 64;                         // destination rows per tile = wgmma M (two A tiles fit next to the W image)
 constexpr int kABufs = 2;
-// Role layout (template parameters EW / GW of the kernel): warps [0, EW) epilogue (TMEM lane quarter = warp & 3, 32-column
-// chunks interleaved by warp >> 2), warp EW = MMA issuer, warps [EW + 1, EW + 1 + GW) gather.  The register file is
+// Role layout (template parameters EW / GW of the kernel): warps [0, EW) MMA + epilogue (warpgroup warp >> 2 takes every
+// (EW / 4)-th 32-column slice), warp EW = W image loader, warps [EW + 1, EW + 1 + GW) gather.  The register file is
 // split evenly over the CTA's threads, so the shape trades gather warps against row loads in flight per lane:
 //   (8, 23) 1024 threads x 64 regs     (4, 19) 768 threads x 80 regs     (4, 11) 512 threads x 128 regs
 constexpr int kMaxGatherWarps = 23;                 // sizes the pointer scratch
@@ -81,7 +82,6 @@ struct SageParams {
   int n_out;                  // real output width
   int relu;
   int out_bf16;
-  int tmem_cols;
   const char* zero_row;       // >= 2 KB of zeros: target of the loads of masked lanes / missing rows
   int wshift_self, wshift_nbr; // log2(world) of each table when it is a power of two, else -1
   // fused softmax cross-entropy (top layer): active when ce_labels != nullptr
@@ -103,7 +103,7 @@ struct SageParams {
 template <int VEC>
 __device__ __forceinline__ void put_chunk(uint8_t* sA, __nv_bfloat16* a_row, int r, int kcol, const float (&v)[VEC]) {
   const int kb = kcol >> 6;
-  const uint32_t off = (uint32_t)kb * (kTileM * 128) + umma::sw128_offset((uint32_t)r, (uint32_t)(kcol & 63));
+  const uint32_t off = (uint32_t)kb * (kTileM * 128) + gmma::sw128_offset((uint32_t)r, (uint32_t)(kcol & 63));
   if constexpr (VEC == 4) {
     uint2 u; u.x = pack_bf16x2(v[0], v[1]); u.y = pack_bf16x2(v[2], v[3]);
     *reinterpret_cast<uint2*>(sA + off) = u;
@@ -127,74 +127,44 @@ __device__ __forceinline__ int find_seg(const SageParams& p, int t) {
 #define GLB_DBG(slot) do { if (p.dbg && lane == 0) p.dbg[(size_t)blockIdx.x * 64 + (slot)] = clock64(); } while (0)
 
 // shared-memory control block (after the pointer buffers)
-enum : int { kBarW = 0, kBarAFull = 1, kBarAFree = 3, kBarTFull = 5, kBarTFree = 7, kNumBars = 9 };
+enum : int { kBarW = 0, kBarAFull = 1, kBarAFree = 3, kNumBars = 5 };
 
 // ------------------------------------------------------------------------------------------------
-// epilogue of one tile: TMEM -> registers -> bias/ReLU -> global (warps 0..3, one row per thread)
+// epilogue of one 32-column slice: wgmma accumulator fragment -> bias/ReLU -> global
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void store_cols32(const SageParams& p, const SageSeg& sg, int m, int n0, const float (&f)[32]) {
-  if (n0 >= p.n_out) return;
-  const bool full = (n0 + 32 <= p.n_out);
+__device__ __forceinline__ void store_pair(const SageParams& p, const SageSeg& sg, int m, int n, float x0, float x1) {
+  if (n >= p.n_out) return;
+  const bool two = n + 1 < p.n_out;
+  const size_t off = (size_t)m * p.out_stride + n;
   if (p.out_bf16) {
-    __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(sg.out) + (size_t)m * p.out_stride + n0;
-    if (full && (p.out_stride & 7) == 0) {
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        uint4 a;
-        a.x = pack_bf16x2(f[8 * i], f[8 * i + 1]); a.y = pack_bf16x2(f[8 * i + 2], f[8 * i + 3]);
-        a.z = pack_bf16x2(f[8 * i + 4], f[8 * i + 5]); a.w = pack_bf16x2(f[8 * i + 6], f[8 * i + 7]);
-        reinterpret_cast<uint4*>(o)[i] = a;
-      }
-    } else {
-#pragma unroll
-      for (int i = 0; i < 32; ++i)
-        if (n0 + i < p.n_out) o[i] = __float2bfloat16(f[i]);
-    }
+    __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(sg.out) + off;
+    if (two && (off & 1) == 0) { *reinterpret_cast<uint32_t*>(o) = pack_bf16x2(x0, x1); return; }
+    o[0] = __float2bfloat16(x0);
+    if (two) o[1] = __float2bfloat16(x1);
   } else {
-    float* o = reinterpret_cast<float*>(sg.out) + (size_t)m * p.out_stride + n0;
-    if (full && (p.out_stride & 3) == 0) {
+    float* o = reinterpret_cast<float*>(sg.out) + off;
+    if (two && (off & 1) == 0) { *reinterpret_cast<float2*>(o) = make_float2(x0, x1); return; }
+    o[0] = x0;
+    if (two) o[1] = x1;
+  }
+}
+
+// d = the m64n32 accumulator of output columns [n0, n0 + 32) of the tile; bias staged once per CTA in shared memory
+// (fp32 [N], zero beyond n_out).  Warp wq of the warpgroup holds rows 16 wq + lane / 4 and 16 wq + lane / 4 + 8.
+__device__ __forceinline__ void sage_epilogue_slice(const SageParams& p, const SageSeg& sg, const float* sBias, const float (&d)[16],
+                                                    int m0, int rows, int n0, int wq, int lane) {
+  const int r0 = wq * 16 + (lane >> 2);
 #pragma unroll
-      for (int i = 0; i < 8; ++i)
-        reinterpret_cast<float4*>(o)[i] = make_float4(f[4 * i], f[4 * i + 1], f[4 * i + 2], f[4 * i + 3]);
-    } else {
+  for (int j = 0; j < 4; ++j) {
+    const int n = n0 + 8 * j + 2 * (lane & 3);
+    const float2 b = *reinterpret_cast<const float2*>(sBias + n);
 #pragma unroll
-      for (int i = 0; i < 32; ++i)
-        if (n0 + i < p.n_out) o[i] = f[i];
+    for (int h = 0; h < 2; ++h) {
+      const int r = r0 + 8 * h;
+      float x0 = d[4 * j + 2 * h] + b.x, x1 = d[4 * j + 2 * h + 1] + b.y;
+      if (p.relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
+      if (r < rows) store_pair(p, sg, m0 + r, n, x0, x1);
     }
-  }
-}
-
-// bias vector staged once per CTA in shared memory (fp32 [N], zero beyond n_out)
-__device__ __forceinline__ void load_cols32(const SageParams& p, const float* sBias, uint32_t taddr, int n0, float (&f)[32]) {
-  uint32_t v[32];
-  umma::tmem_ld32(taddr + (uint32_t)n0, v);
-  umma::tmem_ld_wait();
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const float4 b = *reinterpret_cast<const float4*>(sBias + n0 + 4 * i);     // same address for all lanes: broadcast
-    float x0 = __uint_as_float(v[4 * i]) + b.x, x1 = __uint_as_float(v[4 * i + 1]) + b.y;
-    float x2 = __uint_as_float(v[4 * i + 2]) + b.z, x3 = __uint_as_float(v[4 * i + 3]) + b.w;
-    if (p.relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); x2 = fmaxf(x2, 0.f); x3 = fmaxf(x3, 0.f); }
-    f[4 * i] = x0; f[4 * i + 1] = x1; f[4 * i + 2] = x2; f[4 * i + 3] = x3;
-  }
-}
-
-// phase A of the epilogue: TMEM -> registers -> bias/ReLU -> global.  Eight warps: lane quarter q = warp & 3,
-// 32-column chunks interleaved between the two warps (warp >> 2) that share a quarter.
-__device__ __forceinline__ void sage_epilogue_tile(const SageParams& p, const SageSeg& sg, const float* sBias, uint32_t tmem_acc,
-                                                   int m0, int rows, int warp, int lane, int epi_warps) {
-  // UMMA M = 64: accumulator row r lives in TMEM lane (r / 16) * 32 + (r % 16), i.e. lanes 0..15 of every quarter
-  const int q = warp & 3, half = warp >> 2;
-  if (q * 16 >= rows) return;                          // warp-uniform: this lane quarter holds no valid row
-  const int row = q * 16 + lane;
-  const int m = m0 + row;
-  const bool row_ok = lane < 16 && row < rows;
-  const uint32_t taddr = tmem_acc + ((uint32_t)(q * 32) << 16);
-  for (int n0 = half * 32; n0 < p.N; n0 += 8 * epi_warps) {
-    if (n0 >= p.n_out) break;                          // padded output columns are never read back
-    float f[32];
-    load_cols32(p, sBias, taddr, n0, f);
-    if (row_ok && sg.out) store_cols32(p, sg, m, n0, f);
   }
 }
 
@@ -325,7 +295,7 @@ __device__ __forceinline__ void write_item_ptrs(const SageParams& p, const TileC
 // A tile.
 template <int U, int DT, int EW, int GW>
 __global__ void __launch_bounds__((EW + 1 + GW) * 32, 1) sage_persist_kernel(const __grid_constant__ SageParams p) {
-  constexpr int kEpiWarps = EW, kMmaWarp = EW, kGatherWarp0 = EW + 1, kGatherWarps = GW;
+  constexpr int kEpiWarps = EW, kWWarp = EW, kGatherWarp0 = EW + 1, kGatherWarps = GW;
   if (p.dbg && threadIdx.x == 0) {
     unsigned long long gt; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt));
     p.dbg[(size_t)blockIdx.x * 64 + 60] = (long long)gt;
@@ -334,7 +304,7 @@ __global__ void __launch_bounds__((EW + 1 + GW) * 32, 1) sage_persist_kernel(con
   // keep every pointer derived from the __shared__ symbol by plain integer offsets so that the
   // compiler emits LDS/STS (a uintptr_t round trip would demote them to generic LD/ST)
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024u - (umma::smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint8_t* smem = smem_raw + ((1024u - (gmma::smem_u32(smem_raw) & 1023u)) & 1023u);
   const int k_total = p.kp_self + p.kp_nbr;
   const int nkb = k_total >> 6;
   uint8_t* sA = smem;
@@ -344,53 +314,67 @@ __global__ void __launch_bounds__((EW + 1 + GW) * 32, 1) sage_persist_kernel(con
   const char** sScr = reinterpret_cast<const char**>(sW + (size_t)nkb * w_kb_bytes);   // [kGatherWarps][kScrCap]
   float* sBias = reinterpret_cast<float*>(sScr + kMaxGatherWarps * kScrCap);           // [256]
   uint64_t* bars = reinterpret_cast<uint64_t*>(sBias + 256);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + kNumBars);
 
   const int tid = threadIdx.x;
   const int warp = tid >> 5;
   const int lane = tid & 31;
 
   if (tid == 0) {
-    umma::mbar_init(bars + kBarW, 1);
+    gmma::mbar_init(bars + kBarW, 1);
     for (int i = 0; i < 2; ++i) {
-      umma::mbar_init(bars + kBarAFull + i, kGatherWarps);
-      umma::mbar_init(bars + kBarAFree + i, 1);
-      umma::mbar_init(bars + kBarTFull + i, 1);
-      umma::mbar_init(bars + kBarTFree + i, kEpiWarps);
+      gmma::mbar_init(bars + kBarAFull + i, kGatherWarps);
+      gmma::mbar_init(bars + kBarAFree + i, kEpiWarps);
     }
-    umma::fence_barrier_init();
+    gmma::fence_barrier_init();
   }
   const int img = (int)blockIdx.x % p.n_imgs;
   // (multi-image launches: image `img` owns the output columns [img * N, img * N + N) and the matching bias slice)
   if (tid < 256) sBias[tid] = (p.bias && tid < p.n_out && img * p.N + tid < p.bias_len) ? __ldg(p.bias + img * p.N + tid) : 0.f;
-  if (warp == kMmaWarp) {
-    umma::tmem_alloc(tmem_slot, (uint32_t)p.tmem_cols);
-    umma::tmem_relinquish();
-  }
-  umma::tc_fence_before();
   __syncthreads();
-  umma::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   const int tile_first = (int)blockIdx.x / p.n_imgs, tile_stride = (int)gridDim.x / p.n_imgs;
   if (warp == 0) GLB_DBG(0);
 
   if (warp < kEpiWarps) {
-    // =================================================================== epilogue warps
+    // =================================================================== MMA + epilogue warpgroup(s)
+    const int wgi = warp >> 2, n_wg = kEpiWarps / 4, wq = warp & 3;
+    gmma::mbar_wait(bars + kBarW, 0);
+    const uint32_t w_base = gmma::smem_u32(sW);
+    // padded output columns are never read back: slices past n_out are not computed
+    const int n_slices = (min(p.N, (p.n_out + 31) & ~31)) >> 5;
     int it = 0;
     for (int t = tile_first; t < p.total_tiles; t += tile_stride, ++it) {
-      const int acc = it & 1;
-      umma::mbar_wait(bars + kBarTFull + acc, (uint32_t)((it >> 1) & 1));
-      umma::tc_fence_after();
+      const int buf = it & 1;
+      gmma::mbar_wait(bars + kBarAFull + buf, (uint32_t)((it >> 1) & 1));
       if (warp == 0 && it < 4) GLB_DBG(4 + it * 2);
       const int s = find_seg(p, t);
       SageSeg sg = p.seg[s];
       if (sg.out) sg.out += (size_t)img * p.N * (p.out_bf16 ? 2 : 4);
       const int m0 = (t - sg.tile0) * sg.R;
       const int rows = min(sg.R, sg.M - m0);
-      sage_epilogue_tile(p, sg, sBias, tmem_base + (uint32_t)(acc * p.N), m0, rows, warp, lane, kEpiWarps);
-      umma::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) umma::mbar_arrive(bars + kBarTFree + acc);
+      const uint32_t a_base = gmma::smem_u32(sA + (size_t)buf * a_buf_bytes);
+      if (wgi >= n_slices) {                              // no slice for this warpgroup: the A tile is free right away
+        __syncwarp();
+        if (lane == 0) gmma::mbar_arrive(bars + kBarAFree + buf);
+      }
+      for (int sl = wgi; sl < n_slices; sl += n_wg) {
+        float d[16];
+        gmma::wgmma_fence();
+        for (int kb = 0; kb < nkb; ++kb) {
+          const uint32_t a_kb = a_base + (uint32_t)kb * (kTileM * 128);
+          const uint32_t b_kb = w_base + (uint32_t)kb * w_kb_bytes + (uint32_t)sl * (32 * 128);
+#pragma unroll
+          for (int k4 = 0; k4 < 4; ++k4)
+            gmma::mma_m64n32_bf16<0, 0>(d, gmma::make_desc_sw128(a_kb + k4 * 32), gmma::make_desc_sw128(b_kb + k4 * 32), (kb | k4) ? 1u : 0u);
+        }
+        gmma::wgmma_commit();
+        gmma::wgmma_wait<0>();
+        gmma::fence_regs(d);
+        if (sl + n_wg >= n_slices) {                      // this warp's last MMA on the A tile has completed
+          __syncwarp();
+          if (lane == 0) gmma::mbar_arrive(bars + kBarAFree + buf);
+        }
+        if (sg.out) sage_epilogue_slice(p, sg, sBias, d, m0, rows, sl * 32, wq, lane);
+      }
       if (p.ce_labels != nullptr) {
         __threadfence_block();
         asm volatile("bar.sync 1, %0;" ::"r"(kEpiWarps * 32) : "memory");     // logits of the tile are written
@@ -398,41 +382,17 @@ __global__ void __launch_bounds__((EW + 1 + GW) * 32, 1) sage_persist_kernel(con
       }
       if (warp == 0 && it < 4) GLB_DBG(5 + it * 2);
     }
-  } else if (warp == kMmaWarp) {
-    // =================================================================== MMA issuer (+ W image via TMA)
+  } else if (warp == kWWarp) {
+    // =================================================================== W image via TMA
     if (lane == 0) {
-      umma::mbar_arrive_expect_tx(bars + kBarW, (uint32_t)nkb * w_kb_bytes);
+      gmma::mbar_arrive_expect_tx(bars + kBarW, (uint32_t)nkb * w_kb_bytes);
       const uint8_t* src = reinterpret_cast<const uint8_t*>(p.w_img) + (size_t)img * nkb * w_kb_bytes;
       for (int kb = 0; kb < nkb; ++kb)
-        umma::bulk_g2s(sW + (size_t)kb * w_kb_bytes, src + (size_t)kb * w_kb_bytes, w_kb_bytes, bars + kBarW);
+        gmma::bulk_g2s(sW + (size_t)kb * w_kb_bytes, src + (size_t)kb * w_kb_bytes, w_kb_bytes, bars + kBarW);
     }
     __syncwarp();
-    umma::mbar_wait(bars + kBarW, 0);
+    gmma::mbar_wait(bars + kBarW, 0);
     GLB_DBG(1);
-    const uint32_t idesc = umma::make_idesc_bf16(kTileM, p.N);
-    int it = 0;
-    for (int t = tile_first; t < p.total_tiles; t += tile_stride, ++it) {
-      const int acc = it & 1;
-      umma::mbar_wait(bars + kBarAFull + acc, (uint32_t)((it >> 1) & 1));
-      umma::mbar_wait(bars + kBarTFree + acc, (uint32_t)(((it >> 1) & 1) ^ 1));
-      umma::tc_fence_after();
-      if (it < 4) GLB_DBG(12 + it * 2);
-      if (lane == 0) {
-        const uint32_t d = tmem_base + (uint32_t)(acc * p.N);
-        for (int kb = 0; kb < nkb; ++kb) {
-          const uint32_t a_base = umma::smem_u32(sA + (size_t)acc * a_buf_bytes + (size_t)kb * (kTileM * 128));
-          const uint32_t b_base = umma::smem_u32(sW + (size_t)kb * w_kb_bytes);
-#pragma unroll
-          for (int k4 = 0; k4 < 4; ++k4)
-            umma::mma_bf16_ss(d, umma::make_desc_sw128(a_base + k4 * 32), umma::make_desc_sw128(b_base + k4 * 32), idesc,
-                              (kb | k4) ? 1u : 0u);
-        }
-        umma::mma_commit(bars + kBarAFree + acc);     // this A buffer may be overwritten
-        umma::mma_commit(bars + kBarTFull + acc);     // the accumulator may be drained
-      }
-      __syncwarp();
-      if (it < 4) GLB_DBG(13 + it * 2);
-    }
   } else {
     // =================================================================== gather warps
     constexpr int VEC = Chunk<DT>::kVec;
@@ -464,8 +424,8 @@ __global__ void __launch_bounds__((EW + 1 + GW) * 32, 1) sage_persist_kernel(con
     // tile's phase (a fresh barrier passes the parity-1 wait, so tiles 0 and 1 need no special case)
     auto arrive_upto = [&](int upto) {
       while (arrived < upto) {
-        umma::mbar_wait(bars + kBarAFree + (arrived & 1), (uint32_t)(((arrived >> 1) & 1) ^ 1));
-        if (lane == 0) umma::mbar_arrive(bars + kBarAFull + (arrived & 1));
+        gmma::mbar_wait(bars + kBarAFree + (arrived & 1), (uint32_t)(((arrived >> 1) & 1) ^ 1));
+        if (lane == 0) gmma::mbar_arrive(bars + kBarAFull + (arrived & 1));
         ++arrived;
       }
     };
@@ -543,7 +503,7 @@ __global__ void __launch_bounds__((EW + 1 + GW) * 32, 1) sage_persist_kernel(con
       }
       // ---- A buffer it & 1 may only be written once the MMA of tile it-2 has consumed it
       arrive_upto(it);
-      umma::mbar_wait(bars + kBarAFree + (it & 1), (uint32_t)(((it >> 1) & 1) ^ 1));
+      gmma::mbar_wait(bars + kBarAFree + (it & 1), (uint32_t)(((it >> 1) & 1) ^ 1));
       uint8_t* sAt = sA + (size_t)(it & 1) * a_buf_bytes;
       if (row_ok) {
         const int m = cur.m0 + r;
@@ -559,9 +519,9 @@ __global__ void __launch_bounds__((EW + 1 + GW) * 32, 1) sage_persist_kernel(con
         }
       }
       if (!nvalid || nit != it) {                         // last item of this warp in tile `it`
-        umma::fence_proxy_async_smem();                   // generic-proxy st.shared -> visible to tcgen05 (async proxy)
+        gmma::fence_proxy_async_smem();                   // generic-proxy st.shared -> visible to wgmma (async proxy)
         __syncwarp();
-        if (lane == 0) umma::mbar_arrive(bars + kBarAFull + (it & 1));
+        if (lane == 0) gmma::mbar_arrive(bars + kBarAFull + (it & 1));
         arrived = it + 1;
         if (gw == 0 && it < 4) GLB_DBG(30 + it * 3);
       }
@@ -574,10 +534,8 @@ __global__ void __launch_bounds__((EW + 1 + GW) * 32, 1) sage_persist_kernel(con
     }
     arrive_upto(n_tiles_cta);
   }
-  umma::tc_fence_before();
   __syncthreads();
   if (warp == 0) GLB_DBG(2);
-  if (warp == kMmaWarp) umma::tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols);
   if (p.dbg && threadIdx.x == 0) {
     unsigned long long gt; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt));
     p.dbg[(size_t)blockIdx.x * 64 + 62] = (long long)gt;
@@ -722,8 +680,8 @@ static void plan_tiles(SageParams& p, int64_t rows_forced) {
   p.total_tiles = tiles;
 }
 
-static int g_variant = 2;      // role layout of the persistent kernel (see the table at the top): (4, 19) measured fastest
-                               // at 1 and 2 GPUs (profiles/r2_role_layouts.txt); sage_set_variant / GLB_SAGE_VARIANT override
+static int g_variant = 2;      // role layout of the persistent kernel (see the table at the top): (4, 19) by default;
+                               // sage_set_variant / GLB_SAGE_VARIANT override
 void sage_set_variant(int64_t v) { TORCH_CHECK(v >= 0 && v <= 2, "variant 0..2"); g_variant = (int)v; }
 
 static void launch_persist(SageParams& p, size_t smem, cudaStream_t stream) {
@@ -855,8 +813,6 @@ void sage_fused_multi(const at::Tensor& tself_desc, const at::Tensor& tnbr_desc,
   if (p.out_stride < 0) p.out_stride = n_out;
   p.w_img = w_img.data_ptr();
   p.N = (int)N; p.n_out = (int)n_out; p.relu = relu ? 1 : 0; p.out_bf16 = out_bf16 ? 1 : 0;
-  const int need_cols = 2 * (int)N;
-  p.tmem_cols = need_cols <= 32 ? 32 : need_cols <= 64 ? 64 : need_cols <= 128 ? 128 : need_cols <= 256 ? 256 : 512;
   p.wshift_self = log2_or_neg(p.tself.world);
   p.wshift_nbr = log2_or_neg(p.tnbr.world);
   p.zero_row = zero_row_for(w_img.options(), w_img.get_device());
@@ -920,7 +876,7 @@ std::vector<at::Tensor> sage_fused_forward(const at::Tensor& tself_desc,
 }
 
 // K7 standalone: out = act(A . W^T + b) for a dense bf16 A [M, K] (K multiple of 64, <= 512; N <= 256)
-// on the same persistent tcgen05 / TMEM kernel (the "gather" degenerates to staging A's rows).
+// on the same persistent wgmma kernel (the "gather" degenerates to staging A's rows).
 at::Tensor tc_linear_forward(const at::Tensor& a, const at::Tensor& w_img, const c10::optional<at::Tensor>& bias,
                              int64_t N, int64_t n_out, bool relu, bool out_bf16) {
   TORCH_CHECK(a.is_cuda() && a.scalar_type() == at::kBFloat16 && a.dim() == 2 && a.stride(1) == 1,

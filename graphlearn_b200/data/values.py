@@ -4,7 +4,7 @@
 API parity with graphlearn/python/data/values.py (shapes and property names:
 ``ids [B] | [B,k]``, ``int_attrs/float_attrs/string_attrs [..., n]``,
 ``weights/labels/timestamps``, degrees dicts, ``offsets/indices/dense_shape``
-for sparse objects, 1-based ``Layers.layer_nodes(i)``), but B200-first inside:
+for sparse objects, 1-based ``Layers.layer_nodes(i)``), but GPU-first inside:
 every field is held as a **device tensor** (``.tensor(name)`` / ``.ids_t``) and
 only converted to numpy when the numpy-style property is read, so a training
 loop never bounces a batch through the host.  Attributes are looked up lazily

@@ -2,7 +2,7 @@
 
 The hiactor runtime shards the graph store per core and hands every produced tape to a shard, either round-robin or
 ordered by data size so that shards stay evenly loaded (graphlearn/src/actor/runner/tape_dispatcher.cc:61-175,208-218).
-On B200 the SM grid is the sharded executor, but the dispatch problem is still real one level up: seed traversal is
+On the GPU the SM grid is the sharded executor, but the dispatch problem is still real one level up: seed traversal is
 unsharded (every rank walks the nodes IT owns, node_getter.cc:64-92), so ranks see different batch counts and - with
 skewed degrees - different amounts of sampling / gather work per batch.  ``gl.enable_actor()`` turns on
 :class:`BalancedSeedDispatcher`: at the start of an epoch the ranks exchange their batch weights, a deterministic plan

@@ -5,9 +5,9 @@ path, but forward and backward are an explicit, minimal kernel chain over
 pre-allocated buffers (static shapes -> CUDA graph friendly):
 
   K1    sample hop 1..L of the NEXT batch (parallel branch)            (L launches + 1 counter kernel)
-  K6+K7 ONE persistent launch per layer: gather / aggregate / tcgen05 GEMM of every hop pair of the layer
+  K6+K7 ONE persistent launch per layer: gather / aggregate / wgmma GEMM of every hop pair of the layer
         (multi-segment); the top layer's launch also computes softmax-CE, dlogits and the bias gradient
-  for l = L..1:  dW_l = dZ_l^T A_l   split-K tcgen05 kernel, fp32 accumulation straight into the flat gradient buffer;
+  for l = L..1:  dW_l = dZ_l^T A_l   split-K wgmma kernel, fp32 accumulation straight into the flat gradient buffer;
                                      for l < L, dZ_l = relu'(H_l) * (self + nbr/k rows of dA_{l+1}) is computed by its producers
                  dA_l = dZ_l W_l     the forward kernel with a K-major image of W_l^T                      [l > 1]
   K8    ONE kernel: peer-memory all-reduce (world > 1) + Adam + gradient zeroing + bf16 weight images of the next step
@@ -336,7 +336,7 @@ class FastSageTrainer:
                              top.bias.grad if top.bias is not None else None)
         if self._post_loss_hook is not None:
             self._post_loss_hook()          # e2e graph capture: fork the loss D2H here, parallel to the backward
-        # ---- backward: all GEMMs on tcgen05 (csrc/sage_bwd.cu), no library kernels
+        # ---- backward: all GEMMs on wgmma (csrc/sage_bwd.cu), no library kernels
         #   top layer   : dW_L = dZ_L^T A_L with the dense dZ_L written by the fused loss epilogue
         #   layer l < L : dW_l = dZ_l^T A_l where dZ_l = relu'(H_l) * (self + 1/k neighbour rows of dA_{l+1}) is
         #                 computed inside the GEMM's producer warps (never stored for l = 1); bias grads fall out

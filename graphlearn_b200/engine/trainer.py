@@ -4,7 +4,7 @@ One ``step`` = sample K hops -> fused gather/aggregate/GEMM forward -> loss ->
 backward -> (multi-GPU) peer-memory gradient all-reduce -> fused Adam.  The
 whole step is a stream-ordered chain of device work with static shapes (fixed
 fan-out + padding), so it is captured once into a CUDA graph and replayed:
-this is the B200 replacement for the reference's sampling||training
+this is the GPU replacement for the reference's sampling||training
 producer/consumer pipeline (DagScheduler -> TapeStore -> Dataset prefetch,
 graphlearn/src/core/runner/dag_scheduler.cc:45-86, dag/tape.cc:110-153) -
 there is no host in the loop to overlap with any more.

@@ -2,7 +2,7 @@
 //
 // The reference exposes Client / Server / Dataset / *Request / *Response classes from src/include/
 // (client.h:33-80, server.h:30-60, dag_dataset.h:27-55, tensor.h:35-86); a C++ application links the shared object
-// and drives sampling and lookups without Python.  This header is the equivalent surface for the B200 runtime: a C++
+// and drives sampling and lookups without Python.  This header is the equivalent surface for the GPU runtime: a C++
 // program that links `graphlearn_b200/_C.so` (plus libtorch) gets
 //
 //   glb::api::Graph     in-HBM typed graph of ONE GPU: node tables + CSR topologies built from COO tensors or from the

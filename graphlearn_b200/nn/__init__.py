@@ -1,5 +1,5 @@
 """PyTorch model layer (``gl.nn``): the math of graphlearn/python/nn/tf/* re-implemented as
-torch Modules, with the GraphSAGE layer on the fused sm_100a kernel."""
+torch Modules, with the GraphSAGE layer on the fused sm_90a kernel."""
 from . import loss  # noqa: F401
 from torch.nn import Module  # noqa: F401  (nn/tf/module.py: the base class of every layer / model)
 

@@ -2,7 +2,7 @@
 
 Re-implements the math of the reference's TF1 layers
 (graphlearn/python/nn/tf/layers/ego_{sage,gat,gin,rgcn}_conv.py, SURVEY 2.8)
-with the SAGE layer running on the fused sm_100a kernel.
+with the SAGE layer running on the fused sm_90a kernel.
 """
 from __future__ import annotations
 

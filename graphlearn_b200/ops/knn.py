@@ -4,7 +4,7 @@ The reference wraps faiss indexes (flat / ivfflat / ivfpq, CPU or GPU) behind ``
 broadcast to every server and the per-server top-k lists are merged with a k-heap
 (graphlearn/src/contrib/knn/index_factory.cc:28-50, knn_request.cc:96-111,167-202).  Here:
 
-* **flat** - ``csrc/knn.cu``: one kernel per 128-query tile streams the shard through a tcgen05 score GEMM with a
+* **flat** - ``csrc/knn.cu``: one kernel per 128-query tile streams the shard through a wgmma score GEMM with a
   fused running top-k (the [B, N] score matrix never exists), a second kernel merges the per-SM lists; the
   candidates (2k, scored from bf16 operands) are re-ranked in fp32 so the result equals an fp32 brute force;
 * **ivfflat** - k-means coarse quantiser at build time, inverted lists = a row permutation; a query probes its

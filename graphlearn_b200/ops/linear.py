@@ -1,4 +1,4 @@
-"""K7: dense ``act(x W^T + b)`` on the tcgen05 / TMEM tile kernel (``csrc/sage_fused.cu``,
+"""K7: dense ``act(x W^T + b)`` on the wgmma tile kernel (``csrc/sage_fused.cu``,
 A staged from global memory).  Used by the non-SAGE layers (GAT / GIN / RGCN projections) when
 the shapes fit one tile (K <= 512, out <= 256); otherwise - and on CPU - it is ``F.linear``.
 Backward = two plain library GEMMs.

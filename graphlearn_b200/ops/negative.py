@@ -11,7 +11,7 @@ Semantics follow the reference operators:
   conditional negatives sharing selected attribute values with the positive dst
               (conditional_negative_sampler.cc:37-156)
 
-B200 design: instead of Vose alias tables (alias_method.cc:57-123) the weighted
+GPU design: instead of Vose alias tables (alias_method.cc:57-123) the weighted
 draws use one global inclusive prefix-sum per (shard, distribution) and a
 binary search (``torch.searchsorted`` -> a single vectorised device kernel);
 rejection is a sorted-row membership test against the CSR (rows are fetched

@@ -1,4 +1,4 @@
-"""Fused GraphSAGE layer op (K6+K7): gather -> aggregate -> tcgen05 GEMM -> bias/ReLU.
+"""Fused GraphSAGE layer op (K6+K7): gather -> aggregate -> wgmma GEMM -> bias/ReLU.
 
 Weights are kept in the kernel's padded K layout ``[n_out, kp_self + kp_nbr]``
 (each half padded to 64/128/256/512 columns; pad columns stay zero because

@@ -1,7 +1,7 @@
 """Neighbor sampling ops (K1) - dispatch + portable torch implementation.
 
 ``sample_neighbors`` picks, per call:
-  * the sm_100a peer-memory kernel (csrc/sampling.cu) when the shards live on
+  * the sm_90a peer-memory kernel (csrc/sampling.cu) when the shards live on
     CUDA devices - one launch serves local and remote adjacency rows;
   * otherwise the portable path: hash-partition the seeds, all-to-all them to
     their owners (gloo / NCCL), sample with vectorised torch ops on the local

@@ -7,7 +7,7 @@ each hit is emitted in BOTH directions as (row, col, edge id); with
 ``need_dist`` the SEAL double-radius labels are BFS distances to src (node 0)
 with dst removed and to dst (node 1) with src removed.
 
-B200 design: rows come from the peer-memory full sampler; the intersection is
+GPU design: rows come from the peer-memory full sampler; the intersection is
 a sort + ``searchsorted`` membership test on the device (sorted-set intersect)
 instead of per-row hash maps; BFS is frontier expansion with index ops.
 """

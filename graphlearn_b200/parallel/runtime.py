@@ -5,7 +5,7 @@ naming engine and channel manager (graphlearn/src/service/dist/*.cc, SURVEY
 R14-R18).  One process per GPU; ``torch.distributed`` (NCCL on GPU, gloo on
 CPU) is used ONLY for rendezvous, IPC-handle exchange and as the baseline
 collective path.  Afterwards every rank holds a peer-pointer table for every
-sharded array and the sm_100a kernels dereference peer HBM directly.
+sharded array and the sm_90a kernels dereference peer HBM directly.
 """
 from __future__ import annotations
 

@@ -1,6 +1,6 @@
 """GraphStore: load -> partition -> build the per-GPU shards of a heterogeneous graph.
 
-B200-native counterpart of GraphStore::{Load,Build,BuildStatistics}
+H100-native counterpart of GraphStore::{Load,Build,BuildStatistics}
 (graphlearn/src/core/graph/graph_store.cc:185-333) and of the server Init
 sequence (graphlearn/src/service/server_impl.cc:163-195):
 

@@ -1,6 +1,6 @@
 """Per-GPU graph shards: node tables and CSR adjacency in HBM.
 
-B200-native replacement for the reference's GraphStore / Graph / Noder and the
+H100-native replacement for the reference's GraphStore / Graph / Noder and the
 memory storages (graphlearn/src/core/graph/graph_store.cc:185-333,
 storage/memory_adj_matrix.cc:159-225, memory_node_storage.cc:64-138):
 
@@ -232,8 +232,8 @@ class NodeTable:
         esz = 4 if dtype == torch.float32 else 2
         stride = _round_up(max(d, 1), 16 // esz)
         # rows wider than one 128-byte line start on a line boundary: a 200-byte row then touches exactly 2 lines instead
-        # of 2.6 on average - over NVLink (whole lines travel) that is 23 % fewer bytes, and HBM has room for the padding
-        # (measured: profiles/r2_gather_floor.txt, r2_row_alignment.txt).  `config.feature_row_align` = 16 restores dense rows.
+        # of 2.6 on average - over NVLink (whole lines travel) that is 23 % fewer bytes, and HBM has room for the padding.
+        # `config.feature_row_align` = 16 restores dense rows.
         align = int(getattr(_config.get(), "feature_row_align", 128))
         if align > 16 and d * esz > align // 2:
             stride = _round_up(d * esz, align) // esz
@@ -250,7 +250,7 @@ class NodeTable:
 
         Reference: the optional LFU cache of remote node attributes
         (graphlearn/src/core/graph/storage/remote_node_storage.cc:55-82, cache_policy.h:37-78,
-        enabled by ``set_local_node_cache_capacity``).  B200 design: a STATIC, score-ordered
+        enabled by ``set_local_node_cache_capacity``).  GPU design: a STATIC, score-ordered
         replica (highest global in-degree first, PaGraph style) because a device kernel cannot
         maintain LFU state cheaply and 180 GB of HBM usually holds the whole table; the kernels
         resolve ``vid -> cache slot`` through one int32 map (csrc/host_utils.h TableView).

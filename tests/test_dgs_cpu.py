@@ -677,7 +677,7 @@ def test_reference_dgs_conf_files_load():
     import json
     import os
     from graphlearn_b200.dgs import Options, Schema
-    base = os.path.join(os.environ.get("GLB_REFERENCE_DIR", "/root/reference"), "dynamic_graph_service", "conf")
+    base = os.path.join(os.environ.get("GLB_REFERENCE_DIR", ""), "dynamic_graph_service", "conf")
     if not os.path.isdir(base):
         pytest.skip("no reference checkout")
     want = {"u2i": [("u2i", 10), ("i2i", 5)], "dblp": [("published", 5), ("written", 5)]}

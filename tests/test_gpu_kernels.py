@@ -1,5 +1,5 @@
-"""GPU numerics / semantics tests: every sm_100a kernel against a plain PyTorch
-fp32 reference of the same op (run with ``pytest -m gpu`` on a B200)."""
+"""GPU numerics / semantics tests: every sm_90a kernel against a plain PyTorch
+fp32 reference of the same op (run with ``pytest -m gpu`` on an H100)."""
 import math
 import os
 
@@ -268,7 +268,7 @@ def test_gather_bf16_table(rt):
     dict(M=500, k=3, ds=200, dn=200, n_out=64, mode="mean", relu=True, bf16=False),
 ])
 def test_sage_fused_store_numerics(rt, cfg):
-    """tcgen05 fused layer reading a (fp32) store vs fp32 torch reference."""
+    """wgmma fused layer reading a (fp32) store vs fp32 torch reference."""
     from graphlearn_b200.ops import sage as SG
     from graphlearn_b200.store.shards import IdMap, NodeTable
     M, k, ds, dn = cfg["M"], cfg["k"], cfg["ds"], cfg["dn"]
@@ -310,7 +310,7 @@ def _int_table(rt, n, d, dtype, seed):
 @pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16])
 @pytest.mark.parametrize("M,k,d,n_out", [(300, 10, 100, 256), (25600, 10, 100, 256), (1000, 25, 64, 128), (77, 3, 256, 47)])
 def test_sage_fused_exact_rows(rt, M, k, d, n_out, dtype):
-    """Exact-equality check of the persistent fused kernel (gather + sum + tcgen05 GEMM) on integer data."""
+    """Exact-equality check of the persistent fused kernel (gather + sum + wgmma GEMM) on integer data."""
     from graphlearn_b200.ops import sage as SG
     n = 50000
     t, g = _int_table(rt, n, d, dtype, 1)
@@ -444,7 +444,7 @@ def test_sage_fused_multi_segment_and_ce(rt):
 
 
 def test_bwd_dw_tcgen05(rt):
-    """dW = dZ^T A on the tensor cores (MN-major UMMA operands, split-K, red.global.add) vs torch fp32;
+    """dW = dZ^T A on the tensor cores (MN-major wgmma operands, split-K, red.global.add) vs torch fp32;
     then the fused variant whose dZ is computed from (H, dA_next) inside the GEMM."""
     from graphlearn_b200.parallel.runtime import native
     C = native()
@@ -673,7 +673,7 @@ def test_negative_sampler_kernel(rt, graph):
 
 @pytest.mark.parametrize("M,K,N", [(1000, 100, 47), (4096, 256, 256), (130, 512, 64), (20000, 64, 128)])
 def test_tc_linear(rt, M, K, N):
-    """standalone tcgen05 dense layer (K7) vs fp32 reference, forward and backward."""
+    """standalone wgmma dense layer (K7) vs fp32 reference, forward and backward."""
     from graphlearn_b200.ops.linear import tc_linear
     g = torch.Generator(device=rt.device).manual_seed(M + K)
     x = torch.randn(M, K, device=rt.device, generator=g).to(torch.bfloat16).requires_grad_()

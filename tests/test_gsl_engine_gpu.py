@@ -156,7 +156,7 @@ def test_dgs_kernels_match_cpu_service():
 
 @pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16])
 def test_knn_fused_kernel_flat_and_ivf(dtype):
-    """csrc/knn.cu: tcgen05 score GEMM + fused running top-k + merge; recall@k = 1.0 vs an fp32 brute force."""
+    """csrc/knn.cu: wgmma score GEMM + fused running top-k + merge; recall@k = 1.0 vs an fp32 brute force."""
     import graphlearn_b200 as gl
     from graphlearn_b200.ops import knn
     from graphlearn_b200.parallel.runtime import init
@@ -187,6 +187,27 @@ def test_knn_fused_kernel_flat_and_ivf(dtype):
     ids, _ = knn.search(rt, t, q[:64], k, 0)
     hit = (ids[:, :, None] == ref_i[:64, None, :]).any(2).float().mean()
     assert hit > 0.5, float(hit)
+
+
+def test_knn_flat_wide_queries_single_slab_buffer():
+    """256-wide queries leave shared memory for one database slab only: the flat scan then loads and scores the slabs
+    one after the other, with recall 1.0 vs an fp32 brute force like the double-buffered scan."""
+    from graphlearn_b200.ops import knn
+    from graphlearn_b200.parallel.runtime import init
+    from graphlearn_b200.store.shards import IdMap, NodeTable
+    rt = init()
+    g = torch.Generator(device=rt.device).manual_seed(6)
+    n, d, B, k = 20001, 256, 200, 10
+    x = torch.randn(n, d, device=rt.device, generator=g)
+    t = NodeTable(rt, "t", IdMap(rt, torch.arange(n, device=rt.device), dense=True))
+    t.set_float(x, torch.bfloat16)
+    xs = t.feats.local[:, :d].float()
+    q = torch.randn(B, d, device=rt.device, generator=g)
+    for metric in (0, 1):
+        ids, _ = knn.search(rt, t, q, k, metric)
+        sc = q @ xs.t() if metric == 1 else -torch.cdist(q, xs) ** 2
+        ref_i = torch.topk(sc, k, dim=1).indices
+        assert torch.equal(torch.sort(ids, 1).values, torch.sort(ref_i, 1).values), metric
 
 
 @pytest.mark.parametrize("dtype,d,H,k", [(torch.bfloat16, 100, 4, 10), (torch.float32, 64, 2, 7), (torch.bfloat16, 256, 4, 25)])

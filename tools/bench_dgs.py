@@ -1,6 +1,6 @@
 """DGS benchmark against the reference's published numbers (docs/en/dgs/intro.md:25-29: 2-hop query P99 <= 20 ms,
 20,000 QPS, 110 MB/s update ingest on a 64-core node): streaming ingest throughput, 2-hop query latency and QPS of
-the HBM-resident sampler service on one B200."""
+the HBM-resident sampler service on one H100."""
 import json
 import os
 import sys

@@ -1,4 +1,4 @@
-"""KNN search throughput (K10): flat scan (tcgen05 score GEMM + fused top-k) and IVF-flat on N x d database vectors, recall@k
+"""KNN search throughput (K10): flat scan (wgmma score GEMM + fused top-k) and IVF-flat on N x d database vectors, recall@k
 against an fp32 brute-force oracle.  1 GPU: `python tools/bench_knn.py`; N GPUs: torchrun (database sharded by id % world,
 peer-memory k-way merge)."""
 import json

@@ -1,5 +1,5 @@
-"""Diagnostic for the tcgen05 fused SAGE kernel: structured inputs that expose
-layout mistakes (swizzle, descriptor, TMEM mapping) as recognisable patterns."""
+"""Diagnostic for the wgmma fused SAGE kernel: structured inputs that expose
+layout mistakes (swizzle, descriptor, accumulator fragment mapping) as recognisable patterns."""
 import sys, os, math
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -33,7 +33,7 @@ def run(M, k, d, n_out, mode="mean", w=None, xs=None, xn=None, tag=""):
     return y, ref
 
 
-# 1) identity weights: out[m, n] = x_self[m, n]  (n < 64) -> exposes A/B/TMEM mapping
+# 1) identity weights: out[m, n] = x_self[m, n]  (n < 64) -> exposes A/B/accumulator mapping
 d = 64
 w = torch.zeros(64, 2 * d, device=dev)
 w[torch.arange(64), torch.arange(64)] = 1.0

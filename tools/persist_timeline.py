@@ -20,23 +20,23 @@ for _ in range(3):
 torch.cuda.synchronize()
 NAMES = {0: "start", 1: "W image ready", 2: "cta end"}
 for i in range(4):
-    NAMES[4 + 2 * i] = "epi%d begin" % i; NAMES[5 + 2 * i] = "epi%d end" % i
-    NAMES[12 + 2 * i] = "mma%d begin (A full)" % i; NAMES[13 + 2 * i] = "mma%d issued" % i
+    NAMES[4 + 2 * i] = "mma+epi%d begin (A full)" % i; NAMES[5 + 2 * i] = "mma+epi%d end" % i
     NAMES[20 + 2 * i] = "stage%d begin" % i; NAMES[21 + 2 * i] = "stage%d end" % i
     NAMES[28 + 3 * i] = "gather%d ptrs ready" % i; NAMES[29 + 3 * i] = "gather%d items done (warp 7)" % i
     NAMES[30 + 3 * i] = "gather%d arrived" % i
 
 
 def traced(fn, label):
-    buf = torch.zeros(148 * 64, dtype=torch.int64, device=rt.device)
+    n_sm = torch.cuda.get_device_properties(rt.device).multi_processor_count
+    buf = torch.zeros(n_sm * 64, dtype=torch.int64, device=rt.device)
     C.sage_set_debug_trace(buf)
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     ev0.record(); fn(); ev1.record()
     torch.cuda.synchronize()
     C.sage_set_debug_trace(None)
-    t = buf.view(148, 64).cpu()
+    t = buf.view(n_sm, 64).cpu()
     print("==== %s: %.1f us (CUDA events)" % (label, ev0.elapsed_time(ev1) * 1e3))
-    for cta in (0, 1, 73, 147):
+    for cta in (0, 1, n_sm // 2, n_sm - 1):
         row = t[cta]
         if int(row[0]) == 0:
             continue
