@@ -25,36 +25,28 @@ void sparse_adam_rows(const at::Tensor&, const at::Tensor&, const at::Tensor&, c
                       double, int64_t);
 void gather_copy16(const at::Tensor&, const at::Tensor&, int64_t, const at::Tensor&, bool, int64_t);
 // sage_fused.cu
-int64_t sage_pad_k(int64_t);
 int64_t sage_smem_bytes(int64_t, int64_t);
-at::Tensor pack_weight_sw128(const at::Tensor&, int64_t);
 std::vector<at::Tensor> sage_fused_forward(const at::Tensor&, const c10::optional<at::Tensor>&, const at::Tensor&,
                                            const c10::optional<at::Tensor>&, int64_t, int64_t, int64_t,
                                            const at::Tensor&, const c10::optional<at::Tensor>&, int64_t, int64_t,
-                                           bool, bool, bool, int64_t, const c10::optional<at::Tensor>&,
-                                           const c10::optional<at::Tensor>&);
+                                           bool, bool, bool);
 void sage_fused_multi(const at::Tensor&, const at::Tensor&, const std::vector<c10::optional<at::Tensor>>&,
                       const std::vector<c10::optional<at::Tensor>>&, const std::vector<int64_t>&, const std::vector<int64_t>&,
                       const std::vector<int64_t>&, const std::vector<int64_t>&, const std::vector<at::Tensor>&,
                       const std::vector<c10::optional<at::Tensor>>&, int64_t, const at::Tensor&,
-                      const c10::optional<at::Tensor>&, int64_t, int64_t, bool, bool, int64_t,
-                      const std::vector<c10::optional<at::Tensor>>&, int64_t, int64_t);
+                      const c10::optional<at::Tensor>&, int64_t, int64_t, bool, bool,
+                      const std::vector<c10::optional<at::Tensor>>&, int64_t, int64_t, int64_t);
 int sm_count();
 void sage_set_debug_trace(const c10::optional<at::Tensor>&);
-void sage_set_max_ctas(int64_t);
-void sage_set_variant(int64_t);
 // sage_bwd.cu
 at::Tensor pack_weight_t(const at::Tensor&, int64_t, int64_t);
 void sage_bwd_dw(const c10::optional<at::Tensor>&, const c10::optional<at::Tensor>&, const std::vector<int64_t>&,
                  const std::vector<int64_t>&, const std::vector<c10::optional<at::Tensor>>&,
                  const std::vector<c10::optional<at::Tensor>>&, const std::vector<int64_t>&, const std::vector<double>&, int64_t,
-                 const c10::optional<at::Tensor>&, const at::Tensor&, const at::Tensor&, const c10::optional<at::Tensor>&, int64_t,
-                 const std::vector<int64_t>&);
+                 const c10::optional<at::Tensor>&, const at::Tensor&, const at::Tensor&, const c10::optional<at::Tensor>&, int64_t);
 // train_ops.cu
 void softmax_ce(const at::Tensor&, const at::Tensor&, const c10::optional<at::Tensor>&, int64_t, const at::Tensor&,
                 const at::Tensor&, const c10::optional<at::Tensor>&);
-void sage_bwd_input(const c10::optional<at::Tensor>&, const c10::optional<at::Tensor>&, int64_t, int64_t, double,
-                    const c10::optional<at::Tensor>&, const at::Tensor&, const c10::optional<at::Tensor>&);
 std::vector<at::Tensor> pack_weight_f32(const at::Tensor&, int64_t, bool);
 at::Tensor tc_linear_forward(const at::Tensor&, const at::Tensor&, const c10::optional<at::Tensor>&, int64_t, int64_t, bool,
                              bool);
@@ -175,21 +167,16 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("scatter_add_rows", &glb::scatter_add_rows);
   m.def("gather_copy16", &glb::gather_copy16);
   m.def("sparse_adam_rows", &glb::sparse_adam_rows);
-  m.def("sage_pad_k", &glb::sage_pad_k);
   m.def("sage_smem_bytes", &glb::sage_smem_bytes);
-  m.def("pack_weight_sw128", &glb::pack_weight_sw128);
   m.def("sage_fused_forward", &glb::sage_fused_forward);
   m.def("sage_fused_multi", &glb::sage_fused_multi);
   m.def("sm_count", &glb::sm_count);
   m.def("sage_set_debug_trace", &glb::sage_set_debug_trace);
-  m.def("sage_set_max_ctas", &glb::sage_set_max_ctas);
-  m.def("sage_set_variant", &glb::sage_set_variant);
   m.def("pack_weight_t", &glb::pack_weight_t);
   m.def("sage_bwd_dw", &glb::sage_bwd_dw);
   m.def("pack_weight_f32", &glb::pack_weight_f32);
   m.def("tc_linear_forward", &glb::tc_linear_forward);
   m.def("softmax_ce", &glb::softmax_ce);
-  m.def("sage_bwd_input", &glb::sage_bwd_input);
   m.def("symm_alloc", &glb::symm_alloc);
   m.def("symm_free", &glb::symm_free);
   m.def("ipc_get_handle", &glb::ipc_get_handle);

@@ -11,7 +11,7 @@
 // buffer with vectorised red.global.add (the gradient buffer is zeroed once per step).
 //
 // The dZ operand is usually not read but COMPUTED on the fly (fused "backward through ReLU + mean
-// aggregation", the former sage_bwd_input kernel):
+// aggregation"):
 //     dZ_l[r, :] = relu'(H_l[r, :]) * ( dA_{l+1}[self row of r, 0:d]  +  scale * dA_{l+1}[parent of r, kp_self : kp_self + d] )
 // so dZ of the big hop segments never exists in HBM for 2-layer models; the bias gradient (column sums of
 // dZ) falls out of the same registers.  Deeper models can ask for dZ to be written (needed by dA = dZ.W).
@@ -64,7 +64,6 @@ struct DwParams {
   int rows, n_out, dz_cols, n_cols;
   int m_blocks, n_blocks, rows_per_split;
   uint32_t lbo, sbo, kadv;                  // MN-major descriptor fields (bytes)
-  int skip_red;                             // debug: skip the red.global epilogue
 };
 
 __device__ __forceinline__ uint4 ldg16(const void* p) { return *reinterpret_cast<const uint4*>(p); }
@@ -246,7 +245,7 @@ __global__ void __launch_bounds__(kDwThreads, 1) sage_bwd_dw_kernel(const __grid
     atomicAdd(p.dbias + mb * 128 + tid, v);
   }
   // ------------------------------------------------------------------ epilogue: registers -> red.global.add into dW
-  if (n_steps > 0 && wg_active && !p.skip_red) {
+  if (n_steps > 0 && wg_active) {
     const int r0 = mh * 64 + wq * 16 + (lane >> 2);
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
@@ -312,7 +311,7 @@ void sage_bwd_dw(const c10::optional<at::Tensor>& dz, const c10::optional<at::Te
                  const std::vector<c10::optional<at::Tensor>>& self_src, const std::vector<c10::optional<at::Tensor>>& nbr_src,
                  const std::vector<int64_t>& seg_k, const std::vector<double>& seg_scale, int64_t nbr_col0,
                  const c10::optional<at::Tensor>& dz_out, const at::Tensor& a, const at::Tensor& dw,
-                 const c10::optional<at::Tensor>& dbias, int64_t n_out, const std::vector<int64_t>& desc_override) {
+                 const c10::optional<at::Tensor>& dbias, int64_t n_out) {
   TORCH_CHECK(a.is_cuda() && a.scalar_type() == at::kBFloat16 && a.dim() == 2 && a.stride(1) == 1 && a.stride(0) % 8 == 0);
   TORCH_CHECK(dw.is_cuda() && dw.scalar_type() == at::kFloat && dw.dim() == 2 && dw.stride(1) == 1 && dw.size(0) >= n_out &&
               dw.size(1) == a.size(1) && dw.stride(0) % 4 == 0 && (reinterpret_cast<uintptr_t>(dw.data_ptr()) & 15) == 0,
@@ -378,8 +377,6 @@ void sage_bwd_dw(const c10::optional<at::Tensor>& dz, const c10::optional<at::Te
   p.rows_per_split = rps;
   const int splits = (p.rows + rps - 1) / rps;
   p.lbo = 8192; p.sbo = 1024; p.kadv = 2048;
-  if (desc_override.size() == 4) p.skip_red = (int)desc_override[3];
-  if (desc_override.size() >= 3) { p.lbo = (uint32_t)desc_override[0]; p.sbo = (uint32_t)desc_override[1]; p.kadv = (uint32_t)desc_override[2]; }
   const size_t smem = 1024 + (size_t)kDwStages * kDwStageBytes + 512 + 2 * kDwStages * 8;
   static bool attr_done = false;
   if (!attr_done) {

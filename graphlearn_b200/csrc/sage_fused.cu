@@ -8,7 +8,7 @@
 // tiles cost about the same number of row fetches and the tile count is a multiple of the SM count.
 // Inside the CTA the phases of a tile overlap instead of running back to back:
 //
-//   gather warps (GW, default 19)   each warp owns work items (1-4 destination rows x one 512-byte slice): it
+//   gather warps (19)         each warp owns work items (1-4 destination rows x one 512-byte slice): it
 //                             translates the item's ids into row pointers (local HBM, a peer GPU's HBM over
 //                             NVLink, or the local replica cache) in a private SMEM scratch - the ids of the
 //                             NEXT item are prefetched while the current rows are in flight -, pulls the self
@@ -18,14 +18,13 @@
 //                             ACROSS tile boundaries so no warp idles; the A tile is double buffered; rows may be
 //                             fp32, bf16 or block-scaled fp8 (dequantised while accumulating)
 //   W warp (1)                W image fetched ONCE per CTA by the TMA engine (cp.async.bulk)
-//   MMA + epilogue warps (EW, default 4 = one warpgroup)  per 32-column slice of the output: wgmma
+//   MMA + epilogue warpgroup (4 warps)  per 32-column slice of the output: wgmma
 //                             (M=64, N=32, K=16) over the whole K with the fp32 accumulator in registers,
 //                             then bias -> ReLU -> bf16/fp32 store, while the gather warps are already
 //                             filling the other A buffer with tile t+1; an mbarrier arrival after the last
-//                             slice's MMAs frees the A tile.  Two warpgroups (EW = 8) take alternate slices.
-//                             For the top layer a second, coalesced phase (one warp per row, one lane per
-//                             class) computes the softmax cross-entropy loss, dlogits and the bias gradient
-//                             (fused CE)
+//                             slice's MMAs frees the A tile.  For the top layer a second, coalesced phase
+//                             (one warp per row, one lane per class) computes the softmax cross-entropy
+//                             loss, dlogits and the bias gradient (fused CE)
 //
 // The rows never round-trip through HBM ("agg(X).W" instead of materialising [B*k, D]).
 //
@@ -45,11 +44,14 @@ namespace glb {
 
 constexpr int kTileM = 64;                         // destination rows per tile = wgmma M (two A tiles fit next to the W image)
 constexpr int kABufs = 2;
-// Role layout (template parameters EW / GW of the kernel): warps [0, EW) MMA + epilogue (warpgroup warp >> 2 takes every
-// (EW / 4)-th 32-column slice), warp EW = W image loader, warps [EW + 1, EW + 1 + GW) gather.  The register file is
-// split evenly over the CTA's threads, so the shape trades gather warps against row loads in flight per lane:
-//   (8, 23) 1024 threads x 64 regs     (4, 19) 768 threads x 80 regs     (4, 11) 512 threads x 128 regs
-constexpr int kMaxGatherWarps = 23;                 // sizes the pointer scratch
+// Role layout: warps [0, 4) = the MMA + epilogue warpgroup, warp 4 = W image loader, warps [5, 24) gather.  The register
+// file is split evenly over the CTA's threads, so the layout trades gather warps against row loads in flight per lane:
+// 768 threads get 80 registers each, enough for ptxas to issue a whole batch of U loads back to back.
+constexpr int kEpiWarps = 4;
+constexpr int kWWarp = kEpiWarps;
+constexpr int kGatherWarp0 = kEpiWarps + 1;
+constexpr int kGatherWarps = 19;
+constexpr int kThreads = (kEpiWarps + 1 + kGatherWarps) * 32;
 constexpr int kMaxSegs = 4;
 constexpr int kScrCap = 64;                        // row pointers per gather warp (private scratch): rows_per_item * (k + 1) <= 64
 constexpr size_t kSmemLimit = 232448;
@@ -170,11 +172,11 @@ __device__ __forceinline__ void sage_epilogue_slice(const SageParams& p, const S
 
 // phase B (top layer only): softmax cross-entropy of the tile's rows, one warp per row, lanes = classes
 // (n_out <= 64: columns lane and lane + 32), reading the logits phase A has just written (L2).
-__device__ __forceinline__ void sage_ce_tile(const SageParams& p, const SageSeg& sg, int m0, int rows, int warp, int lane, int epi_warps) {
+__device__ __forceinline__ void sage_ce_tile(const SageParams& p, const SageSeg& sg, int m0, int rows, int warp, int lane) {
   const float* logits = reinterpret_cast<const float*>(sg.out);
   const int c0 = lane, c1 = lane + 32;
   float db0 = 0.f, db1 = 0.f, lsum = 0.f;
-  for (int r = warp; r < rows; r += epi_warps) {
+  for (int r = warp; r < rows; r += kEpiWarps) {
     const int m = m0 + r;
     const float* lrow = logits + (size_t)m * p.out_stride;
     const float x0 = c0 < p.n_out ? __ldcg(lrow + c0) : -FLT_MAX;
@@ -293,9 +295,8 @@ __device__ __forceinline__ void write_item_ptrs(const SageParams& p, const TileC
 // 32-lane slices.  Per item a lane group issues ALL self + neighbour chunk loads of a batch
 // unconditionally (masked lanes read a zero row), reduces in fp32 and writes bf16 into the SW128
 // A tile.
-template <int U, int DT, int EW, int GW>
-__global__ void __launch_bounds__((EW + 1 + GW) * 32, 1) sage_persist_kernel(const __grid_constant__ SageParams p) {
-  constexpr int kEpiWarps = EW, kWWarp = EW, kGatherWarp0 = EW + 1, kGatherWarps = GW;
+template <int U, int DT>
+__global__ void __launch_bounds__(kThreads, 1) sage_persist_kernel(const __grid_constant__ SageParams p) {
   if (p.dbg && threadIdx.x == 0) {
     unsigned long long gt; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt));
     p.dbg[(size_t)blockIdx.x * 64 + 60] = (long long)gt;
@@ -312,7 +313,7 @@ __global__ void __launch_bounds__((EW + 1 + GW) * 32, 1) sage_persist_kernel(con
   uint8_t* sW = sA + (size_t)kABufs * a_buf_bytes;
   const uint32_t w_kb_bytes = (uint32_t)p.N * 128u;
   const char** sScr = reinterpret_cast<const char**>(sW + (size_t)nkb * w_kb_bytes);   // [kGatherWarps][kScrCap]
-  float* sBias = reinterpret_cast<float*>(sScr + kMaxGatherWarps * kScrCap);           // [256]
+  float* sBias = reinterpret_cast<float*>(sScr + kGatherWarps * kScrCap);              // [256]
   uint64_t* bars = reinterpret_cast<uint64_t*>(sBias + 256);
 
   const int tid = threadIdx.x;
@@ -335,8 +336,7 @@ __global__ void __launch_bounds__((EW + 1 + GW) * 32, 1) sage_persist_kernel(con
   if (warp == 0) GLB_DBG(0);
 
   if (warp < kEpiWarps) {
-    // =================================================================== MMA + epilogue warpgroup(s)
-    const int wgi = warp >> 2, n_wg = kEpiWarps / 4, wq = warp & 3;
+    // =================================================================== MMA + epilogue warpgroup
     gmma::mbar_wait(bars + kBarW, 0);
     const uint32_t w_base = gmma::smem_u32(sW);
     // padded output columns are never read back: slices past n_out are not computed
@@ -352,11 +352,7 @@ __global__ void __launch_bounds__((EW + 1 + GW) * 32, 1) sage_persist_kernel(con
       const int m0 = (t - sg.tile0) * sg.R;
       const int rows = min(sg.R, sg.M - m0);
       const uint32_t a_base = gmma::smem_u32(sA + (size_t)buf * a_buf_bytes);
-      if (wgi >= n_slices) {                              // no slice for this warpgroup: the A tile is free right away
-        __syncwarp();
-        if (lane == 0) gmma::mbar_arrive(bars + kBarAFree + buf);
-      }
-      for (int sl = wgi; sl < n_slices; sl += n_wg) {
+      for (int sl = 0; sl < n_slices; ++sl) {
         float d[16];
         gmma::wgmma_fence();
         for (int kb = 0; kb < nkb; ++kb) {
@@ -369,16 +365,17 @@ __global__ void __launch_bounds__((EW + 1 + GW) * 32, 1) sage_persist_kernel(con
         gmma::wgmma_commit();
         gmma::wgmma_wait<0>();
         gmma::fence_regs(d);
-        if (sl + n_wg >= n_slices) {                      // this warp's last MMA on the A tile has completed
+        if (sl == n_slices - 1) {                         // this warp's last MMA on the A tile has completed
           __syncwarp();
           if (lane == 0) gmma::mbar_arrive(bars + kBarAFree + buf);
         }
-        if (sg.out) sage_epilogue_slice(p, sg, sBias, d, m0, rows, sl * 32, wq, lane);
+        // (warp < 4 here; the mask tells the compiler so: without it the <6, bf16> instantiation spills at 80 registers)
+        if (sg.out) sage_epilogue_slice(p, sg, sBias, d, m0, rows, sl * 32, warp & 3, lane);
       }
       if (p.ce_labels != nullptr) {
         __threadfence_block();
         asm volatile("bar.sync 1, %0;" ::"r"(kEpiWarps * 32) : "memory");     // logits of the tile are written
-        sage_ce_tile(p, sg, m0, rows, warp, lane, kEpiWarps);
+        sage_ce_tile(p, sg, m0, rows, warp, lane);
       }
       if (warp == 0 && it < 4) GLB_DBG(5 + it * 2);
     }
@@ -542,22 +539,6 @@ __global__ void __launch_bounds__((EW + 1 + GW) * 32, 1) sage_persist_kernel(con
   }
 }
 
-// bf16 row-major [n_real, k_total] -> SW128 K-major image with N (>= n_real) rows per k-block
-__global__ void pack_sw128_kernel(const __nv_bfloat16* __restrict__ w, int n_real, int N, int k_total,
-                                  uint8_t* __restrict__ img) {
-  int idx = blockIdx.x * blockDim.x + threadIdx.x;   // one 16-byte chunk each
-  int nkb = k_total >> 6;
-  int total = nkb * N * 8;
-  if (idx >= total) return;
-  int c = idx & 7;
-  int n = (idx >> 3) % N;
-  int kb = (idx >> 3) / N;
-  uint4 val = make_uint4(0, 0, 0, 0);
-  if (n < n_real) val = *reinterpret_cast<const uint4*>(w + (size_t)n * k_total + kb * 64 + c * 8);
-  size_t off = (size_t)kb * N * 128 + (size_t)(n >> 3) * 1024 + (size_t)(n & 7) * 128 + (size_t)((c ^ (n & 7)) * 16);
-  *reinterpret_cast<uint4*>(img + off) = val;
-}
-
 // fp32 row-major padded weight [n_real, k_total] -> (SW128 bf16 image, bf16 row-major copy) in one pass
 __global__ void pack_sw128_f32_kernel(const float* __restrict__ w, int n_real, int N, int k_total,
                                       uint8_t* __restrict__ img, __nv_bfloat16* __restrict__ w16) {
@@ -590,32 +571,16 @@ static int pad_k(int d) {
   return 512;
 }
 
-int64_t sage_pad_k(int64_t d) { return pad_k((int)d); }
-
 // dynamic shared memory of the persistent kernel: A tile + W image + per-warp pointer scratch + bias + control + alignment slack
+// (ops/sage.py smem_bytes mirrors this term for term)
 int64_t sage_smem_bytes(int64_t k_total, int64_t N) {
-  return 1024 + kABufs * (k_total / 64) * (kTileM * 128) + (k_total / 64) * N * 128 + kMaxGatherWarps * kScrCap * 8 + 256 * 4 + (kNumBars + 2) * 8;
+  return 1024 + kABufs * (k_total / 64) * (kTileM * 128) + (k_total / 64) * N * 128 + kGatherWarps * kScrCap * 8 + 256 * 4 + (kNumBars + 2) * 8;
 }
 
 int sm_count() {
   static int n = 0;
   if (n == 0) n = at::cuda::getCurrentDeviceProperties()->multiProcessorCount;
   return n;
-}
-
-at::Tensor pack_weight_sw128(const at::Tensor& w_padded, int64_t N) {
-  TORCH_CHECK(w_padded.is_cuda() && w_padded.scalar_type() == at::kBFloat16 && w_padded.dim() == 2 &&
-              w_padded.is_contiguous(), "w_padded must be a contiguous CUDA bf16 [n, k_total] tensor");
-  int64_t n_real = w_padded.size(0), k_total = w_padded.size(1);
-  TORCH_CHECK(k_total % 64 == 0 && N % 8 == 0 && N >= n_real, "bad padded weight shape");
-  c10::cuda::CUDAGuard guard(w_padded.device());
-  auto img = at::empty({(k_total / 64) * N * 64}, w_padded.options());
-  int total = (int)((k_total / 64) * N * 8);
-  pack_sw128_kernel<<<(total + 255) / 256, 256, 0, at::cuda::getCurrentCUDAStream()>>>(
-      reinterpret_cast<const __nv_bfloat16*>(w_padded.data_ptr()), (int)n_real, (int)N, (int)k_total,
-      reinterpret_cast<uint8_t*>(img.data_ptr()));
-  C10_CUDA_KERNEL_LAUNCH_CHECK();
-  return img;
 }
 
 // returns (image, bf16 row-major copy)
@@ -639,9 +604,6 @@ std::vector<at::Tensor> pack_weight_f32(const at::Tensor& w_padded, int64_t N, b
 }
 
 static long long* g_dbg_ptr = nullptr;
-static int g_max_ctas = 0;     // 0 = all SMs; engines cap a launch that should co-run with another whole-SM kernel
-void sage_set_max_ctas(int64_t n) { g_max_ctas = (int)n; }
-static int usable_sms() { const int s = sm_count(); return g_max_ctas > 0 ? std::min(s, g_max_ctas) : s; }
 void sage_set_debug_trace(const c10::optional<at::Tensor>& t) {
   g_dbg_ptr = (t.has_value() && t->defined()) ? reinterpret_cast<long long*>(t->data_ptr<int64_t>()) : nullptr;
 }
@@ -656,8 +618,8 @@ static const char* zero_row_for(const at::TensorOptions& opts, int dev) {
 
 // Balanced tiling: every tile should cost about the same number of row fetches ((k + 1) per destination
 // row, + 2 for the epilogue / A stores) and the tile count should just fill `waves` tiles per SM.
-static void plan_tiles(SageParams& p, int64_t rows_forced) {
-  const int sms = std::max(1, usable_sms() / p.n_imgs);
+static void plan_tiles(SageParams& p, int usable_sms) {
+  const int sms = std::max(1, usable_sms / p.n_imgs);
   int64_t n128 = 0;
   double total_cost = 0.0;
   for (int s = 0; s < p.nseg; ++s) {
@@ -671,7 +633,6 @@ static void plan_tiles(SageParams& p, int64_t rows_forced) {
     SageSeg& sg = p.seg[s];
     int64_t R = (int64_t)std::ceil(target / (double)(sg.k + 3));
     R = (R + 7) / 8 * 8;
-    if (rows_forced > 0) R = (rows_forced + 7) / 8 * 8;
     R = std::min<int64_t>(kTileM, std::max<int64_t>(8, R));
     sg.R = (int)R;
     sg.tile0 = tiles;
@@ -680,41 +641,25 @@ static void plan_tiles(SageParams& p, int64_t rows_forced) {
   p.total_tiles = tiles;
 }
 
-static int g_variant = 2;      // role layout of the persistent kernel (see the table at the top): (4, 19) by default;
-                               // sage_set_variant / GLB_SAGE_VARIANT override
-void sage_set_variant(int64_t v) { TORCH_CHECK(v >= 0 && v <= 2, "variant 0..2"); g_variant = (int)v; }
-
-static void launch_persist(SageParams& p, size_t smem, cudaStream_t stream) {
+static void launch_persist(SageParams& p, size_t smem, int usable_sms, cudaStream_t stream) {
   if (p.total_tiles == 0) return;
-  const unsigned grid = (unsigned)(p.n_imgs * std::min<int>(std::max(1, usable_sms() / p.n_imgs), p.total_tiles));
+  const unsigned grid = (unsigned)(p.n_imgs * std::min<int>(std::max(1, usable_sms / p.n_imgs), p.total_tiles));
   int kmax = 1;
   for (int s = 0; s < p.nseg; ++s) kmax = std::max(kmax, p.seg[s].k);
   const int dt = p.tnbr.dtype;
-#define LAUNCH(UU, DD, EW, GW)                                                                             \
+#define LAUNCH(UU, DD)                                                                                     \
   do {                                                                                                     \
     static bool attr_done = false;                                                                         \
     if (!attr_done) {                                                                                      \
-      C10_CUDA_CHECK(cudaFuncSetAttribute(sage_persist_kernel<UU, DD, EW, GW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemLimit)); \
+      C10_CUDA_CHECK(cudaFuncSetAttribute(sage_persist_kernel<UU, DD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemLimit)); \
       attr_done = true;                                                                                    \
     }                                                                                                      \
-    sage_persist_kernel<UU, DD, EW, GW><<<grid, (EW + 1 + GW) * 32, smem, stream>>>(p);                    \
+    sage_persist_kernel<UU, DD><<<grid, kThreads, smem, stream>>>(p);                                      \
   } while (0)
-#define LAUNCH_DT(UU, EW, GW) do { if (dt == 0) LAUNCH(UU, 0, EW, GW); else LAUNCH(UU, 1, EW, GW); } while (0)
-#define LAUNCH_DT3(UU, EW, GW) do { if (dt == 2) LAUNCH(UU, 2, EW, GW); else LAUNCH_DT(UU, EW, GW); } while (0)
-  TORCH_CHECK(dt != 2 || g_variant == 2, "fp8 feature rows are built for the default role layout only");
-  if (g_variant == 1) {
-    // 512 threads x 128 registers: a whole neighbour list (or half of a long one) in flight per lane
-    const int u = kmax <= 5 ? 5 : kmax <= 10 ? 10 : 13;
-    if (u == 5) LAUNCH_DT(5, 4, 11); else if (u == 10) LAUNCH_DT(10, 4, 11); else LAUNCH_DT(13, 4, 11);
-  } else if (g_variant == 2) {
-    const int u = kmax <= 4 ? 4 : (kmax % 5 == 0 || kmax > 12) ? 5 : 6;
-    if (u == 4) LAUNCH_DT3(4, 4, 19); else if (u == 5) LAUNCH_DT3(5, 4, 19); else LAUNCH_DT3(6, 4, 19);
-  } else {
-    const int u = kmax <= 4 ? 4 : (kmax % 5 == 0 || kmax > 12) ? 5 : 6;
-    if (u == 4) LAUNCH_DT(4, 8, 23); else if (u == 5) LAUNCH_DT(5, 8, 23); else LAUNCH_DT(6, 8, 23);
-  }
+#define LAUNCH_DT3(UU) do { if (dt == 2) LAUNCH(UU, 2); else if (dt == 0) LAUNCH(UU, 0); else LAUNCH(UU, 1); } while (0)
+  const int u = kmax <= 4 ? 4 : (kmax % 5 == 0 || kmax > 12) ? 5 : 6;
+  if (u == 4) LAUNCH_DT3(4); else if (u == 5) LAUNCH_DT3(5); else LAUNCH_DT3(6);
 #undef LAUNCH_DT3
-#undef LAUNCH_DT
 #undef LAUNCH
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
@@ -725,6 +670,7 @@ static void launch_persist(SageParams& p, size_t smem, cudaStream_t stream) {
 // a_saves[i] ([M_i, K_total] bf16, the [self || agg] rows for the backward pass).
 // ce = optional fused softmax cross-entropy on the output rows of segment 0:
 //   [labels_table(int64), seeds(int64)|undefined, loss(fp32 >=1), dlogits(bf16 [M, stride]), dbias(fp32)|undefined]
+// max_ctas caps the grid (0 = one CTA per SM), leaving SMs to a kernel that should run beside this launch.
 void sage_fused_multi(const at::Tensor& tself_desc, const at::Tensor& tnbr_desc,
                       const std::vector<c10::optional<at::Tensor>>& self_vids,
                       const std::vector<c10::optional<at::Tensor>>& nbr_vids,
@@ -732,8 +678,8 @@ void sage_fused_multi(const at::Tensor& tself_desc, const at::Tensor& tnbr_desc,
                       const std::vector<int64_t>& Ms, const std::vector<int64_t>& ks,
                       const std::vector<at::Tensor>& outs, const std::vector<c10::optional<at::Tensor>>& a_saves,
                       int64_t mode, const at::Tensor& w_img, const c10::optional<at::Tensor>& bias, int64_t N,
-                      int64_t n_out, bool relu, bool out_bf16, int64_t rows_forced,
-                      const std::vector<c10::optional<at::Tensor>>& ce, int64_t ce_world, int64_t n_imgs) {
+                      int64_t n_out, bool relu, bool out_bf16,
+                      const std::vector<c10::optional<at::Tensor>>& ce, int64_t ce_world, int64_t n_imgs, int64_t max_ctas) {
   TORCH_CHECK(w_img.is_cuda() && w_img.scalar_type() == at::kBFloat16, "w_img must be CUDA bf16");
   c10::cuda::CUDAGuard guard(w_img.device());
   const int nseg = (int)Ms.size();
@@ -844,8 +790,9 @@ void sage_fused_multi(const at::Tensor& tself_desc, const at::Tensor& tnbr_desc,
     p.ce_inv_b = 1.f / (float)Ms[0];
   }
   p.dbg = g_dbg_ptr;
-  plan_tiles(p, rows_forced);
-  launch_persist(p, smem, at::cuda::getCurrentCUDAStream());
+  const int usable_sms = max_ctas > 0 ? std::min<int>(sm_count(), (int)max_ctas) : sm_count();
+  plan_tiles(p, usable_sms);
+  launch_persist(p, smem, usable_sms, at::cuda::getCurrentCUDAStream());
 }
 
 // single-segment convenience wrapper (autograd op in ops/sage.py)
@@ -855,23 +802,20 @@ std::vector<at::Tensor> sage_fused_forward(const at::Tensor& tself_desc,
                                            const c10::optional<at::Tensor>& nbr_vids, int64_t M,
                                            int64_t k, int64_t mode, const at::Tensor& w_img,
                                            const c10::optional<at::Tensor>& bias, int64_t N,
-                                           int64_t n_out, bool relu, bool out_bf16, bool save_a, int64_t rows_per_cta,
-                                           const c10::optional<at::Tensor>& out_buf,
-                                           const c10::optional<at::Tensor>& a_buf) {
+                                           int64_t n_out, bool relu, bool out_bf16, bool save_a) {
   c10::cuda::CUDAGuard guard(w_img.device());
   auto opts = w_img.options();
-  at::Tensor out = out_buf.has_value() && out_buf->defined() ? *out_buf
-                                                             : at::empty({M, n_out}, opts.dtype(out_bf16 ? at::kBFloat16 : at::kFloat));
+  at::Tensor out = at::empty({M, n_out}, opts.dtype(out_bf16 ? at::kBFloat16 : at::kFloat));
   at::Tensor a_save;
   if (save_a) {
     const TableView ts = table_from_desc(tself_desc), tn = table_from_desc(tnbr_desc);
     const int64_t k_total = ((mode == kGcnMean) ? 0 : pad_k(ts.dim)) + (k > 0 ? pad_k(tn.dim) : 0);
-    a_save = a_buf.has_value() && a_buf->defined() ? *a_buf : at::empty({M, k_total}, opts.dtype(at::kBFloat16));
+    a_save = at::empty({M, k_total}, opts.dtype(at::kBFloat16));
   }
   if (M == 0) return {out, a_save};
   sage_fused_multi(tself_desc, tnbr_desc, {self_vids}, {nbr_vids}, {0}, {0}, {M}, {k}, {out},
                    {save_a ? c10::optional<at::Tensor>(a_save) : c10::nullopt}, mode, w_img, bias, N, n_out, relu, out_bf16,
-                   rows_per_cta, {}, 1, 1);
+                   {}, 1, 1, 0);
   return {out, a_save};
 }
 
@@ -890,7 +834,7 @@ at::Tensor tc_linear_forward(const at::Tensor& a, const at::Tensor& w_img, const
   d[0] = 1; d[1] = K; d[2] = a.stride(0); d[3] = 1; d[4] = M; d[4 + kMaxWorld] = reinterpret_cast<int64_t>(a.data_ptr());
   at::Tensor desc = at::from_blob(d.data(), {(int64_t)d.size()}, at::kLong).clone();
   sage_fused_multi(desc, desc, {c10::nullopt}, {c10::nullopt}, {0}, {0}, {M}, {0}, {out}, {c10::nullopt}, kConcatMean, w_img, bias,
-                   N, n_out, relu, out_bf16, 0, {}, 1, 1);
+                   N, n_out, relu, out_bf16, {}, 1, 1, 0);
   return out;
 }
 

@@ -5,12 +5,6 @@
 //  * softmax_ce_kernel     logits -> mean cross-entropy loss, dlogits (bf16,
 //                          already scaled by 1/B) and the bias gradient
 //                          (column sums) in ONE single-CTA kernel.
-//  * sage_bwd_input_kernel dA of layer l  ->  dZ of layer l-1: adds the "self"
-//                          and the "neighbour" (1/k broadcast) contributions
-//                          of every hop row, applies the ReLU mask of the
-//                          saved activations, writes bf16 and accumulates the
-//                          bias gradient - a gather formulation, no atomics on
-//                          the activations and no zero-fill pass.
 // Loss parity: graphlearn/python/nn/tf/loss.py (softmax cross entropy).
 #include <torch/extension.h>
 #include <ATen/cuda/CUDAContext.h>
@@ -56,125 +50,6 @@ softmax_ce_kernel(const float* __restrict__ logits, int ld_logits, const int64_t
     for (int c = threadIdx.x; c < C; c += blockDim.x) atomicAdd(dbias + c, colsum[c]);
 }
 
-// out[r, :d] = relu'(h[r]) * ( self_src ? dA_self[r, 0:d] : 0  +  nbr_src ? dA_nbr[r / k, kp_self : kp_self+d] * scale : 0 )
-// one warp per row; 8-byte (4 x bf16) chunks per lane
-__global__ void __launch_bounds__(256)
-sage_bwd_input_kernel(const __nv_bfloat16* __restrict__ dA_self, const __nv_bfloat16* __restrict__ dA_nbr,
-                      int64_t ld_da, int kp_self, int k, float scale, const __nv_bfloat16* __restrict__ h,
-                      int64_t ld_h, __nv_bfloat16* __restrict__ out, int64_t ld_out, int64_t n_rows, int d,
-                      float* __restrict__ dbias) {
-  extern __shared__ float colsum[];      // [d]
-  for (int c = threadIdx.x; c < d; c += blockDim.x) colsum[c] = 0.f;
-  __syncthreads();
-  const int lane = threadIdx.x & 31;
-  const int64_t warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-  const int chunks = d >> 2;             // d % 4 == 0
-  for (int c0 = 0; c0 < chunks; c0 += 32) {
-    const int c = c0 + lane;
-    float4 cs = make_float4(0.f, 0.f, 0.f, 0.f);
-    for (int64_t r = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < n_rows; r += warps) {
-      if (c >= chunks) continue;
-      float4 g = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (dA_self) {
-        uint2 u = *reinterpret_cast<const uint2*>(dA_self + (size_t)r * ld_da + 4 * c);
-        float2 a = unpack_bf16x2(u.x), b = unpack_bf16x2(u.y);
-        g.x += a.x; g.y += a.y; g.z += b.x; g.w += b.y;
-      }
-      if (dA_nbr) {
-        uint2 u = *reinterpret_cast<const uint2*>(dA_nbr + (size_t)(r / k) * ld_da + kp_self + 4 * c);
-        float2 a = unpack_bf16x2(u.x), b = unpack_bf16x2(u.y);
-        g.x += a.x * scale; g.y += a.y * scale; g.z += b.x * scale; g.w += b.y * scale;
-      }
-      if (h) {
-        uint2 u = *reinterpret_cast<const uint2*>(h + (size_t)r * ld_h + 4 * c);
-        float2 a = unpack_bf16x2(u.x), b = unpack_bf16x2(u.y);
-        if (!(a.x > 0.f)) g.x = 0.f;
-        if (!(a.y > 0.f)) g.y = 0.f;
-        if (!(b.x > 0.f)) g.z = 0.f;
-        if (!(b.y > 0.f)) g.w = 0.f;
-      }
-      uint2 o; o.x = pack_bf16x2(g.x, g.y); o.y = pack_bf16x2(g.z, g.w);
-      *reinterpret_cast<uint2*>(out + (size_t)r * ld_out + 4 * c) = o;
-      cs.x += g.x; cs.y += g.y; cs.z += g.z; cs.w += g.w;
-    }
-    if (dbias && c < chunks) {
-      atomicAdd(&colsum[4 * c], cs.x); atomicAdd(&colsum[4 * c + 1], cs.y);
-      atomicAdd(&colsum[4 * c + 2], cs.z); atomicAdd(&colsum[4 * c + 3], cs.w);
-    }
-  }
-  __syncthreads();
-  if (dbias)
-    for (int c = threadIdx.x; c < d; c += blockDim.x) atomicAdd(dbias + c, colsum[c]);
-}
-
-
-// Same contract, 16-byte (8 x bf16) chunks per lane and U rows in flight per warp: for d = 256 one warp
-// covers a whole row in a single pass and keeps 3*U independent 16-byte loads outstanding (the first
-// version moved 8 bytes per lane with one row in flight and was latency bound: 15.7 us for 27 MB).
-template <int U>
-__global__ void __launch_bounds__(256, 4)
-sage_bwd_input_v8_kernel(const __nv_bfloat16* __restrict__ dA_self, const __nv_bfloat16* __restrict__ dA_nbr,
-                         int64_t ld_da, int kp_self, int k, float scale, const __nv_bfloat16* __restrict__ h,
-                         int64_t ld_h, __nv_bfloat16* __restrict__ out, int64_t ld_out, int64_t n_rows, int d,
-                         float* __restrict__ dbias) {
-  extern __shared__ float colsum[];      // [d]
-  for (int c = threadIdx.x; c < d; c += blockDim.x) colsum[c] = 0.f;
-  __syncthreads();
-  const int lane = threadIdx.x & 31;
-  // 32-bit row arithmetic (the launcher guarantees n_rows < 2^31): `r / k` as a 64-bit division costs
-  // ~100 instructions in front of every neighbour-row load
-  const int warps = (int)((gridDim.x * blockDim.x) >> 5);
-  const int w0 = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
-  const int nr = (int)n_rows;
-  const int chunks = d >> 3;             // d % 8 == 0
-  const uint4 zero4 = make_uint4(0u, 0u, 0u, 0u);
-  for (int c = lane; c < chunks; c += 32) {
-    float cs[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) cs[i] = 0.f;
-    for (int rb = w0; rb < nr; rb += warps * U) {
-      uint4 vs[U], vn[U], vh[U];
-#pragma unroll
-      for (int u = 0; u < U; ++u) {
-        const int r = rb + u * warps;
-        const bool ok = r < nr;
-        vs[u] = (ok && dA_self) ? *reinterpret_cast<const uint4*>(dA_self + (size_t)r * ld_da + 8 * c) : zero4;
-        vn[u] = (ok && dA_nbr) ? *reinterpret_cast<const uint4*>(dA_nbr + (size_t)(r / k) * ld_da + kp_self + 8 * c) : zero4;
-        vh[u] = (ok && h) ? *reinterpret_cast<const uint4*>(h + (size_t)r * ld_h + 8 * c) : zero4;
-      }
-#pragma unroll
-      for (int u = 0; u < U; ++u) {
-        const int r = rb + u * warps;
-        if (r >= nr) continue;
-        const uint32_t* ps = reinterpret_cast<const uint32_t*>(&vs[u]);
-        const uint32_t* pn = reinterpret_cast<const uint32_t*>(&vn[u]);
-        const uint32_t* ph = reinterpret_cast<const uint32_t*>(&vh[u]);
-        uint32_t o[4];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          float2 a = unpack_bf16x2(ps[i]), b = unpack_bf16x2(pn[i]);
-          float gx = a.x + b.x * scale, gy = a.y + b.y * scale;
-          if (h) {
-            float2 hv = unpack_bf16x2(ph[i]);
-            if (!(hv.x > 0.f)) gx = 0.f;
-            if (!(hv.y > 0.f)) gy = 0.f;
-          }
-          o[i] = pack_bf16x2(gx, gy);
-          cs[2 * i] += gx; cs[2 * i + 1] += gy;
-        }
-        *reinterpret_cast<uint4*>(out + (size_t)r * ld_out + 8 * c) = make_uint4(o[0], o[1], o[2], o[3]);
-      }
-    }
-    if (dbias) {
-#pragma unroll
-      for (int i = 0; i < 8; ++i) atomicAdd(&colsum[8 * c + i], cs[i]);
-    }
-  }
-  __syncthreads();
-  if (dbias)
-    for (int c = threadIdx.x; c < d; c += blockDim.x) atomicAdd(dbias + c, colsum[c]);
-}
-
 // ---------------------------------------------------------------------------
 void softmax_ce(const at::Tensor& logits, const at::Tensor& labels_table, const c10::optional<at::Tensor>& seeds,
                 int64_t world, const at::Tensor& loss_accum, const at::Tensor& dlogits,
@@ -195,54 +70,6 @@ void softmax_ce(const at::Tensor& logits, const at::Tensor& labels_table, const 
   softmax_ce_kernel<<<blocks, 256, (size_t)C * sizeof(float), at::cuda::getCurrentCUDAStream()>>>(
       logits.data_ptr<float>(), (int)logits.stride(0), labels_table.data_ptr<int64_t>(), sp, (int)world, B, C, loss_accum.data_ptr<float>(),
       reinterpret_cast<__nv_bfloat16*>(dlogits.data_ptr()), (int)dlogits.stride(0), db);
-  C10_CUDA_KERNEL_LAUNCH_CHECK();
-}
-
-void sage_bwd_input(const c10::optional<at::Tensor>& dA_self, const c10::optional<at::Tensor>& dA_nbr,
-                    int64_t kp_self, int64_t k, double scale, const c10::optional<at::Tensor>& h,
-                    const at::Tensor& out, const c10::optional<at::Tensor>& dbias) {
-  TORCH_CHECK(out.is_cuda() && out.scalar_type() == at::kBFloat16 && out.dim() == 2 && out.stride(1) == 1);
-  c10::cuda::CUDAGuard guard(out.device());
-  int64_t n = out.size(0);
-  int d = (int)out.size(1);
-  TORCH_CHECK(d % 4 == 0, "feature dim must be a multiple of 4");
-  if (n == 0) return;
-  const __nv_bfloat16 *ps = nullptr, *pn = nullptr, *ph = nullptr;
-  int64_t ld_da = 0, ld_h = 0;
-  if (dA_self.has_value()) {
-    TORCH_CHECK(dA_self->scalar_type() == at::kBFloat16 && dA_self->stride(1) == 1 && dA_self->size(0) >= n);
-    ps = reinterpret_cast<const __nv_bfloat16*>(dA_self->data_ptr()); ld_da = dA_self->stride(0);
-  }
-  if (dA_nbr.has_value()) {
-    TORCH_CHECK(dA_nbr->scalar_type() == at::kBFloat16 && dA_nbr->stride(1) == 1 && dA_nbr->size(0) * k >= n);
-    pn = reinterpret_cast<const __nv_bfloat16*>(dA_nbr->data_ptr());
-    TORCH_CHECK(ld_da == 0 || ld_da == dA_nbr->stride(0), "self / nbr dA must share the leading dimension");
-    ld_da = dA_nbr->stride(0);
-  }
-  if (h.has_value()) {
-    TORCH_CHECK(h->scalar_type() == at::kBFloat16 && h->stride(1) == 1 && h->size(0) >= n && h->size(1) == d);
-    ph = reinterpret_cast<const __nv_bfloat16*>(h->data_ptr()); ld_h = h->stride(0);
-  }
-  float* db = nullptr;
-  if (dbias.has_value()) { TORCH_CHECK(dbias->scalar_type() == at::kFloat && dbias->numel() >= d); db = dbias->data_ptr<float>(); }
-  const bool v8 = (d % 8 == 0) && (ld_da % 8 == 0) && (ld_h % 8 == 0) && (out.stride(0) % 8 == 0) && (kp_self % 8 == 0) &&
-                  ((reinterpret_cast<uintptr_t>(out.data_ptr()) & 15) == 0) &&
-                  (!ps || (reinterpret_cast<uintptr_t>(ps) & 15) == 0) && (!pn || (reinterpret_cast<uintptr_t>(pn) & 15) == 0) &&
-                  (!ph || (reinterpret_cast<uintptr_t>(ph) & 15) == 0);
-  if (v8) {
-    constexpr int U = 2;
-    TORCH_CHECK(n < (int64_t)1 << 31, "too many rows");
-    int blocks8 = (int)std::min<int64_t>((int64_t)sm_count() * 4, ((n + U - 1) / U * 32 + 255) / 256);
-    sage_bwd_input_v8_kernel<U><<<blocks8, 256, (size_t)d * sizeof(float), at::cuda::getCurrentCUDAStream()>>>(
-        ps, pn, ld_da, (int)kp_self, (int)std::max<int64_t>(k, 1), (float)scale, ph, ld_h,
-        reinterpret_cast<__nv_bfloat16*>(out.data_ptr()), out.stride(0), n, d, db);
-    C10_CUDA_KERNEL_LAUNCH_CHECK();
-    return;
-  }
-  int blocks = (int)std::min<int64_t>((int64_t)sm_count() * 4, (n * 32 + 255) / 256);
-  sage_bwd_input_kernel<<<blocks, 256, (size_t)d * sizeof(float), at::cuda::getCurrentCUDAStream()>>>(
-      ps, pn, ld_da, (int)kp_self, (int)std::max<int64_t>(k, 1), (float)scale, ph, ld_h,
-      reinterpret_cast<__nv_bfloat16*>(out.data_ptr()), out.stride(0), n, d, db);
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
 

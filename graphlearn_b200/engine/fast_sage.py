@@ -323,13 +323,13 @@ class FastSageTrainer:
                 d = self.nodes.feat_desc
                 C.sage_fused_multi(d, d, [hops[i] for i in range(nseg)], [hops[i + 1] for i in range(nseg)],
                                    [0] * nseg, [0] * nseg, Ms, ks, outs, asv, mode, img, c.bias, N, n_out,
-                                   not last, not last, 0, ce, self.rt.world, ns)
+                                   not last, not last, ce, self.rt.world, ns, 0)
             else:
                 po = self.seg_off[l - 2]
                 d = local_table_desc(self.H[l - 2])
                 C.sage_fused_multi(d, d, [None] * nseg, [None] * nseg, [po[i] for i in range(nseg)],
                                    [po[i + 1] for i in range(nseg)], Ms, ks, outs, asv, mode, img, c.bias, N,
-                                   n_out, not last, not last, 0, ce, self.rt.world, ns)
+                                   n_out, not last, not last, ce, self.rt.world, ns, 0)
             if last and not fuse_ce:
                 # wide / split top layer: the loss runs as its own kernel on the (padded) logits
                 C.softmax_ce(self.H[L - 1], self.nodes.labels.local, seeds, self.rt.world, self.loss, self.dZ[L - 1],
@@ -348,7 +348,7 @@ class FastSageTrainer:
                 sA.wait_stream(main)
                 with torch.cuda.stream(sA):            # dW_L runs beside dA_L
                     C.sage_bwd_dw(self.dZ[l - 1], None, [], [], [], [], [], [], 0, None, a, c.weight_p.grad, None,
-                                  c.out_dim, [])
+                                  c.out_dim)
             else:
                 nxt = self.convs[l]
                 da = self.dA[l]
@@ -364,7 +364,7 @@ class FastSageTrainer:
                           for s in range(nseg)]
                 C.sage_bwd_dw(None, self.H[l - 1], r0, r1, selfs, nbrs, ks, scales, kp_self_n,
                               self.dZ[l - 1] if l >= 2 else None, a, c.weight_p.grad,
-                              c.bias.grad if c.bias is not None else None, c.out_dim, [])
+                              c.bias.grad if c.bias is not None else None, c.out_dim)
             if l >= 2:
                 # dA_l [rows, K_total] = dZ_l [rows, n_out] . W_l, one launch per 256-column block
                 dzp = self.dZp[l - 1]
@@ -375,12 +375,10 @@ class FastSageTrainer:
                 # one launch: CTA b multiplies by image b % n_imgs and writes the columns [256 img, 256 img + 256)
                 n_imgs = wt.size(0)
                 cols = min(256, da.size(1))
-                if l == L:
-                    # dW_L (<= 32 whole-SM CTAs for a 1024-row top layer) runs beside this launch: leave it its SMs
-                    C.sage_set_max_ctas(max(C.sm_count() - 32, C.sm_count() // 2))
+                # dW_L (<= 32 whole-SM CTAs for a 1024-row top layer) runs beside the dA_L launch: leave it its SMs
+                max_ctas = max(C.sm_count() - 32, C.sm_count() // 2) if l == L else 0
                 C.sage_fused_multi(d, d, [None], [None], [0], [0], [rows], [0], [da[:, :cols]], [None], 0, wt, None, 256, cols,
-                                   False, True, 0, [], 1, n_imgs)
-                C.sage_set_max_ctas(0)
+                                   False, True, [], 1, n_imgs, max_ctas)
         # ---- join, gradient all-reduce + fused optimiser (Adam + zero grads + next step's weight images)
         main.wait_stream(sA)
         if pipe is not None:

@@ -55,9 +55,15 @@ def fused_supported(d_self: int, d_nbr: int, n_out: int, mode: str, k: int = 0, 
     return smem_fits(kp_self + kp_nbr, pad_n(n_out))
 
 
+def smem_bytes(k_total: int, n_pad: int) -> int:
+    """Dynamic shared memory of the persistent kernel, term for term as csrc/sage_fused.cu sage_smem_bytes:
+    alignment slack + two A tiles + W image + 19 gather warps x 64 row pointers + bias + control block."""
+    nkb = k_total // 64
+    return 1024 + 2 * nkb * (64 * 128) + nkb * n_pad * 128 + 19 * 64 * 8 + 256 * 4 + (5 + 2) * 8
+
+
 def smem_fits(k_total: int, n_pad: int) -> bool:
-    """A tile + W image + pointer staging of the persistent kernel (csrc/sage_fused.cu sage_smem_bytes)."""
-    return 1024 + (k_total // 64) * (128 * 128 + n_pad * 128) + 23 * 64 * 8 + 1024 + 72 <= _SMEM_LIMIT
+    return smem_bytes(k_total, n_pad) <= _SMEM_LIMIT
 
 
 def logical_weight(weight_p: torch.Tensor, d_self: int, d_nbr: int, mode: str) -> torch.Tensor:
@@ -84,7 +90,7 @@ def _aligned_rows(x: torch.Tensor) -> torch.Tensor:
 class _SageFusedFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, weight_p, bias, x_self, x_nbr, tself_desc, self_vids, tnbr_desc, nbr_vids, M, k, mode,
-                relu, out_bf16, rows_per_cta):
+                relu, out_bf16):
         C = native()
         n_out = weight_p.size(0)
         if x_self is not None:
@@ -101,8 +107,7 @@ class _SageFusedFn(torch.autograd.Function):
         need_x = (x_self is not None and ctx.needs_input_grad[2]) or (x_nbr is not None and ctx.needs_input_grad[3])
         img, w16 = C.pack_weight_f32(weight_p.detach().contiguous(), N, bool(need_x))
         out, a_save = C.sage_fused_forward(tself_desc, self_vids, tnbr_desc, nbr_vids, int(M), int(k), MODE[mode], img,
-                                           bias, N, n_out, bool(relu), bool(out_bf16), bool(need_w),
-                                           int(rows_per_cta), None, None)
+                                           bias, N, n_out, bool(relu), bool(out_bf16), bool(need_w))
         ctx.save_for_backward(a_save if need_w else None, w16 if need_x else None, out if relu else None)
         ctx.meta = (d_self, d_nbr, kp_self, kp_nbr, int(M), int(k), mode, relu, bias is not None,
                     x_self is not None, x_nbr is not None)
@@ -138,7 +143,7 @@ class _SageFusedFn(torch.autograd.Function):
                     scale = (1.0 / k) if mode == "mean" else 1.0
                     dn = da[:, kp_self:kp_self + d_nbr] * scale
                     dxn = dn[:, None, :].expand(M, k, d_nbr).reshape(M * k, d_nbr)
-        return (dw, db, dxs, dxn) + (None,) * 10
+        return (dw, db, dxs, dxn) + (None,) * 9
 
 
 # torch.mm(bf16, bf16, out_dtype=fp32) (CUDA only) writes the fp32 gradient without a cast kernel
@@ -174,7 +179,7 @@ def sage_layer_reference(weight, bias, xs, xn, k, mode="mean", relu=False):
 def sage_layer(weight_p: torch.Tensor, bias: Optional[torch.Tensor], *, k: int, mode: str = "mean",
                relu: bool = False, out_bf16: bool = False, x_self: Optional[torch.Tensor] = None,
                x_nbr: Optional[torch.Tensor] = None, self_table=None, self_vids: Optional[torch.Tensor] = None,
-               nbr_table=None, nbr_vids: Optional[torch.Tensor] = None, rows_per_cta: int = 0) -> torch.Tensor:
+               nbr_table=None, nbr_vids: Optional[torch.Tensor] = None) -> torch.Tensor:
     """One GraphSAGE layer.  ``weight_p`` is in the padded K layout (see module doc).
     Each of {self, nbr} is either a dense local matrix (``x_*``; gradients flow) or
     (:class:`NodeTable`, vids) read from the sharded store inside the kernel."""
@@ -194,7 +199,7 @@ def sage_layer(weight_p: torch.Tensor, bias: Optional[torch.Tensor], *, k: int, 
         return _SageFusedFn.apply(weight_p, bias, x_self, x_nbr,
                                   None if self_table is None else self_table.feat_desc, self_vids,
                                   None if nbr_table is None else nbr_table.feat_desc, nbr_vids,
-                                  M, k, mode, relu, out_bf16, rows_per_cta)
+                                  M, k, mode, relu, out_bf16)
     # portable / unfused path
     xs = x_self if x_self is not None else G.gather_rows(self_table.rt, self_table.feats, self_table.feat_desc,
                                                          self_vids, d_self)

@@ -26,9 +26,6 @@ def native():
     global _NATIVE
     if _NATIVE is None:
         _NATIVE = _build.load()
-        v = os.environ.get("GLB_SAGE_VARIANT")          # role layout of the persistent fused kernel (csrc/sage_fused.cu)
-        if v is not None:
-            _NATIVE.sage_set_variant(int(v))
     return _NATIVE
 
 

@@ -34,6 +34,12 @@ def test_padded_weight_roundtrip():
     assert wp.shape == (7, 256) and torch.equal(SG.logical_weight(wp, 100, 100, "mean"), w)
     assert float(wp[:, 100:128].abs().sum()) == 0 and float(wp[:, 228:].abs().sum()) == 0
     assert SG.fused_supported(100, 100, 256, "mean") and not SG.fused_supported(600, 600, 256, "mean")
+    # the Python fit check and the kernel's launch check size shared memory with the same formula
+    from graphlearn_b200.parallel.runtime import native
+    C = native()
+    for k in (64, 128, 256, 512, 1024):
+        for n in range(32, 257, 32):
+            assert SG.smem_bytes(k, n) == C.sage_smem_bytes(k, n), (k, n)
 
 
 def test_gat_softmax_rows_sum_to_one():

@@ -65,7 +65,7 @@ torch.cuda.synchronize()
 for i, a in enumerate(calls[:3]):
     for rep in range(2):
         traced(lambda: orig(*a), "persistent launch %d (rep %d)" % (i + 1, rep))
-# dW kernel: with and without the red.global epilogue (desc_override[3] = 1 skips the reds)
+# dW kernel launches of one eager step, re-run as they ran
 dw_calls = []
 orig_dw = C.sage_bwd_dw
 def hook_dw(*a):
@@ -76,11 +76,9 @@ tr._skip_opt = True
 tr.step(torch.randint(0, nodes.n_local, (1024,), generator=g))
 torch.cuda.synchronize()
 for a in dw_calls:
-    for ov, label in (([], "with reds"), ([8192, 1024, 2048, 1], "reds skipped")):
-        aa = list(a); aa[-1] = ov
-        ts = []
-        for rep in range(5):
-            ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            ev0.record(); orig_dw(*aa); ev1.record(); torch.cuda.synchronize()
-            ts.append(ev0.elapsed_time(ev1) * 1e3)
-        print("dW launch rows=%d: %s: %s us" % (aa[10].size(0), label, ["%.1f" % x for x in ts]))
+    ts = []
+    for rep in range(5):
+        ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        ev0.record(); orig_dw(*a); ev1.record(); torch.cuda.synchronize()
+        ts.append(ev0.elapsed_time(ev1) * 1e3)
+    print("dW launch rows=%d: %s us" % (a[10].size(0), ["%.1f" % x for x in ts]))
