@@ -20,7 +20,7 @@ std::vector<at::Tensor> sample_full(const at::Tensor&, const at::Tensor&, int64_
 void rng_advance(const at::Tensor&, int64_t);
 at::Tensor random_walk(const at::Tensor&, const at::Tensor&, int64_t, double, double, int64_t, int64_t, const at::Tensor&, int64_t);
 at::Tensor negative_sample(const at::Tensor&, const at::Tensor&, int64_t, const c10::optional<at::Tensor>&, const at::Tensor&, int64_t, bool,
-                           int64_t, int64_t, const at::Tensor&, int64_t);
+                           int64_t, int64_t, const at::Tensor&, int64_t, const c10::optional<at::Tensor>&);
 at::Tensor gather_rows(const at::Tensor&, const at::Tensor&, bool, double);
 std::vector<at::Tensor> load_table(const std::string&, bool, bool, bool, bool, std::vector<int64_t>, std::vector<int64_t>, const std::string&,
                                    const std::string&, int64_t, int64_t, int64_t);
@@ -239,7 +239,7 @@ at::Tensor Graph::NegativeSample(const std::string& edge_type, const at::Tensor&
   c10::optional<at::Tensor> cum;
   if (by_in_degree) cum = at::bincount(t.indices, {}, n_dst).to(at::kDouble).cumsum(0).contiguous();
   return glb::negative_sample(t.desc, ids.to(device_, at::kLong), k, cum, shard_off, n_dst, strict, /*retry=*/3, /*scan_cap=*/512, rng_,
-                              ++salt_);
+                              ++salt_, c10::nullopt);
 }
 
 Stats Graph::GetStats() const {

@@ -16,7 +16,8 @@ at::Tensor random_walk(const at::Tensor&, const at::Tensor&, int64_t, double, do
                        const at::Tensor&, int64_t);
 // negative.cu
 at::Tensor negative_sample(const at::Tensor&, const at::Tensor&, int64_t, const c10::optional<at::Tensor>&,
-                           const at::Tensor&, int64_t, bool, int64_t, int64_t, const at::Tensor&, int64_t);
+                           const at::Tensor&, int64_t, bool, int64_t, int64_t, const at::Tensor&, int64_t,
+                           const c10::optional<at::Tensor>&);
 // gather.cu
 at::Tensor gather_rows(const at::Tensor&, const at::Tensor&, bool, double);
 at::Tensor gather_agg(const at::Tensor&, const at::Tensor&, const c10::optional<at::Tensor>&, int64_t, int64_t);
@@ -47,6 +48,9 @@ void sage_bwd_dw(const c10::optional<at::Tensor>&, const c10::optional<at::Tenso
 // train_ops.cu
 void softmax_ce(const at::Tensor&, const at::Tensor&, const c10::optional<at::Tensor>&, int64_t, const at::Tensor&,
                 const at::Tensor&, const c10::optional<at::Tensor>&);
+void link_loss(const at::Tensor&, int64_t, int64_t, int64_t, double, const at::Tensor&, const at::Tensor&,
+               const c10::optional<at::Tensor>&);
+void link_roots(const at::Tensor&, const at::Tensor&, const at::Tensor&, const at::Tensor&, int64_t, int64_t);
 std::vector<at::Tensor> pack_weight_f32(const at::Tensor&, int64_t, bool);
 at::Tensor tc_linear_forward(const at::Tensor&, const at::Tensor&, const c10::optional<at::Tensor>&, int64_t, int64_t, bool,
                              bool);
@@ -177,6 +181,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("pack_weight_f32", &glb::pack_weight_f32);
   m.def("tc_linear_forward", &glb::tc_linear_forward);
   m.def("softmax_ce", &glb::softmax_ce);
+  m.def("link_loss", &glb::link_loss);
+  m.def("link_roots", &glb::link_roots);
   m.def("symm_alloc", &glb::symm_alloc);
   m.def("symm_free", &glb::symm_free);
   m.def("ipc_get_handle", &glb::ipc_get_handle);

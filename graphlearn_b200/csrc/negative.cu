@@ -66,17 +66,27 @@ __global__ void __launch_bounds__(256) negative_sample_kernel(const CsrView g, c
   p.out[t] = cand;
 }
 
+// `out`: optional preallocated int64 [B * k] (contiguous) the draws are written to, so that the launch allocates
+// nothing and can be captured into a CUDA graph; without it a fresh [B, k] tensor is returned.
 at::Tensor negative_sample(const at::Tensor& csr_desc, const at::Tensor& src, int64_t k,
                            const c10::optional<at::Tensor>& cum, const at::Tensor& shard_off, int64_t n_total,
                            bool strict,
-                           int64_t retry, int64_t scan_cap, const at::Tensor& rng_state, int64_t salt) {
+                           int64_t retry, int64_t scan_cap, const at::Tensor& rng_state, int64_t salt,
+                           const c10::optional<at::Tensor>& out_buf) {
   check_cuda_i64(src, "src");
   check_cuda_i64(shard_off, "shard_off");
   c10::cuda::CUDAGuard guard(src.device());
   CsrView g = csr_from_desc(csr_desc);
   auto s = src.contiguous();
   int64_t B = s.numel();
-  auto out = at::empty({B, k}, s.options());
+  at::Tensor out;
+  if (out_buf.has_value()) {
+    out = *out_buf;
+    check_cuda_i64(out, "out");
+    TORCH_CHECK(out.is_contiguous() && out.numel() == B * k, "out must be a contiguous int64 tensor of B * k elements");
+  } else {
+    out = at::empty({B, k}, s.options());
+  }
   if (B * k == 0) return out;
   NegParams p;
   p.src = s.data_ptr<int64_t>(); p.out = out.data_ptr<int64_t>();

@@ -223,12 +223,16 @@ class FastSageTrainer:
         if self._q_epoch != it.epoch:
             self._q_refresh()
         if self._q_order is None:                       # 'random' traversal: draws with replacement
-            return self.step(self._q_vids[it.next_index()])
+            return self._q_step(self._q_vids[it.next_index()])
         lo = it.cursor
         it.next_index()                                  # advances the cursor / raises OutOfRangeError at the epoch end
         if it.strategy == "shuffle" and lo * 2 > it.n and getattr(self, "_q_thread", None) is None and getattr(self, "_q_next", None) is None:
             self._q_prefetch_epoch(it.epoch + 1)         # randperm of millions of rows costs ~20 ms: off the step path
-        return self.step(self._q_order[lo:lo + self.B])
+        return self._q_step(self._q_order[lo:lo + it.bs])
+
+    def _q_step(self, batch: torch.Tensor) -> torch.Tensor:
+        """train on one batch of the root traversal (here: seed vids)"""
+        return self.step(batch)
 
     def _q_prefetch_epoch(self, epoch: int):
         """build the NEXT epoch's permutation (same generator seeding as SeedIterator) on a host thread"""
@@ -257,6 +261,22 @@ class FastSageTrainer:
             hops.append(cur)
         return hops
 
+    # ------------------------------------------------------------------ what a subclass with other roots / loss replaces
+    _fuse_ce = True         # the top layer's forward launch computes softmax-CE in its epilogue when it fits
+
+    def _stage(self, roots: torch.Tensor, host_slot: int):
+        """captured head of the sampling branch: the staged batch (pinned slot, UVA-mapped) -> root buffer"""
+        self.C.copy_i64(roots, self._h_seeds_dev[host_slot])
+
+    def _draw_roots(self, roots: torch.Tensor):
+        """complete a root buffer whose staged part is in place, before its hops are sampled (here: nothing)"""
+
+    def _top_loss(self, seeds: torch.Tensor):
+        """loss, dZ_L and the top bias gradient from the fp32 top-layer output when it was not fused"""
+        top = self.convs[-1]
+        self.C.softmax_ce(self.H[-1], self.nodes.labels.local, seeds, self.rt.world, self.loss, self.dZ[-1],
+                          top.bias.grad if top.bias is not None else None)
+
     # ------------------------------------------------------------------ the step
     def _step_body(self, pipe=None):
         """One training step as a small DAG of launches.  Independent work runs on forked streams (graph
@@ -275,6 +295,7 @@ class FastSageTrainer:
         if pipe is None:
             # plain schedule: sample this step's batch, then train on it
             seeds = self.seeds
+            self._draw_roots(seeds)
             hops = self.sample(seeds)
             # counters advance once the sampling kernels have consumed the RNG offset; needed again only by Adam
             self.opt.advance(self.rng.state)
@@ -290,8 +311,9 @@ class FastSageTrainer:
             with torch.cuda.stream(sS):
                 if host_slot is not None:
                     # zero-copy staging: a tiny copy KERNEL reads the UVA-mapped pinned buffer over PCIe
-                    C.copy_i64(self._hops[nxt][0], self._h_seeds_dev[host_slot])
+                    self._stage(self._hops[nxt][0], host_slot)
                 nb = self._hops[nxt][0]
+                self._draw_roots(nb)
                 for i, k in enumerate(self.fanouts):
                     S.sample_neighbors(self.csr, nb, k, self.strategy, want_eids=False, rng=self.rng, salt=i + 1,
                                        out=self._hops[nxt][i + 1])
@@ -307,7 +329,7 @@ class FastSageTrainer:
             N = self.n_img[l - 1]
             n_out = c.out_dim if ns == 1 else N
             img = self.img[l - 1]
-            fuse_ce = last and ns == 1 and N <= 64
+            fuse_ce = last and self._fuse_ce and ns == 1 and N <= 64
             offs = self.seg_off[l - 1]
             mode = sage_ops.MODE[c.agg_type]
             nseg = L - l + 1
@@ -332,8 +354,7 @@ class FastSageTrainer:
                                    n_out, not last, not last, ce, self.rt.world, ns, 0)
             if last and not fuse_ce:
                 # wide / split top layer: the loss runs as its own kernel on the (padded) logits
-                C.softmax_ce(self.H[L - 1], self.nodes.labels.local, seeds, self.rt.world, self.loss, self.dZ[L - 1],
-                             top.bias.grad if top.bias is not None else None)
+                self._top_loss(seeds)
         if self._post_loss_hook is not None:
             self._post_loss_hook()          # e2e graph capture: fork the loss D2H here, parallel to the backward
         # ---- backward: all GEMMs on wgmma (csrc/sage_bwd.cu), no library kernels
@@ -471,6 +492,7 @@ class FastSageTrainer:
 
     def _prime_hops(self, seeds: torch.Tensor):
         """Fill BOTH hop buffers with a sample of `seeds` so that whichever graph replays first finds a batch."""
+        self._draw_roots(seeds)
         hops = self.sample(seeds)
         for j in range(2):
             for dst, src in zip(self._hops[j], hops):

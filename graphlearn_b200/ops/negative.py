@@ -139,7 +139,7 @@ def edge_negative(store, etype: str, src_v: torch.Tensor, k: int, strategy: str,
             return torch.full((B, k), -1, dtype=torch.int64, device=dev)
         return native().negative_sample(csr.desc, src_v.reshape(-1), int(k), cum, off, int(total),
                                         strategy == "in_degree", int(cfg.neg_sampling_retry_times), 1024,
-                                        rng.state, int(salt))
+                                        rng.state, int(salt), None)
     if strategy == "random":
         return _draw_global_uniform(dst_tab, B, k, gen, dev)
     if strategy == "in_degree":
