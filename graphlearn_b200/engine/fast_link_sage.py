@@ -66,7 +66,6 @@ class FastLinkSageTrainer(FastSageTrainer):
         self._neg_retry = int(_config.get().neg_sampling_retry_times)
         self._edge_rows = csr._row_of_edge
         self._edge_dst = csr.indices.local
-        self._q_iter = None
 
     def _local_in_degrees(self) -> torch.Tensor:
         """in-degree of every node this rank owns under the edge type (what ``GraphStore.reverse_csr`` counts)"""
@@ -116,8 +115,7 @@ class FastLinkSageTrainer(FastSageTrainer):
         self.C.link_loss(self.H[-1], self.batch_size, self.neg_num, LOSS_KINDS[self.loss_kind], self.temperature,
                          self.loss, self.dZ[-1], top.bias.grad if top.bias is not None else None)
 
-    # ------------------------------------------------------------------ public steps
-    def _fill_slot(self, slot: int, first: torch.Tensor, dst: Optional[torch.Tensor]):
+    def _fill_slot(self, slot: int, first: torch.Tensor, dst: Optional[torch.Tensor] = None):
         """pinned staging slot: [0, B) src vids or CSR positions, [B, 2B) dst vids, [2B] what [0, B) holds"""
         B = self.batch_size
         if first.numel() != B or (dst is not None and dst.numel() != B):
@@ -130,29 +128,12 @@ class FastLinkSageTrainer(FastSageTrainer):
             h[B:2 * B].copy_(dst.reshape(-1))
             h[2 * B] = 0
 
-    def _step_staged(self, first: torch.Tensor, dst: Optional[torch.Tensor]) -> torch.Tensor:
-        if self.graph is not None and getattr(self, "_e2e_graphs", None):
-            # pipelined like FastSageTrainer.step: this call stages its edges, the replay trains on the previous call's
-            i = self._steps & 1
-            self._e2e_done[i].synchronize()    # step t-2 (same graph) was the last reader of staging slot i^1
-            self._fill_slot(i ^ 1, first, dst)
-            if not self._primed:
-                self._stage(self._hops[i][0], i ^ 1)
-                self._prime_hops(self._hops[i][0])
-                self._primed = True
-            self._e2e_graphs[i].replay()
-            self._e2e_done[i].record()
-            self._steps += 1
-            self.h_loss = self._h_loss2[i]
-            return self.h_loss
-        self._e2e_done[0].synchronize()        # the previous eager step's staging kernel has read slot 0
-        self._fill_slot(0, first, dst)
-        self._stage(self.seeds, 0)
-        self._e2e_done[0].record()
-        FastSageTrainer.step_device(self)
-        self.h_loss.copy_(self.loss_out, non_blocking=True)
-        return self.h_loss
+    def _put_roots(self, roots: torch.Tensor, src: torch.Tensor, dst: torch.Tensor):
+        B = self.batch_size
+        self.C.copy_i64(roots[:B], src)
+        self.C.copy_i64(roots[B:2 * B], dst)
 
+    # ------------------------------------------------------------------ public steps
     def step(self, src_ids_host: torch.Tensor, dst_ids_host: torch.Tensor) -> torch.Tensor:
         """End-to-end step on B host edges (src / dst vids).  Asynchronous, and with CUDA graphs pipelined exactly like
         ``FastSageTrainer.step``: the call stages its edges and trains on those of the previous call; the returned
@@ -162,31 +143,14 @@ class FastLinkSageTrainer(FastSageTrainer):
     def step_edges(self) -> torch.Tensor:
         """One step on the next B local edges of the edge traversal ``E(t).batch(B).shuffle(traverse=True)``: every
         local edge once per epoch, full batches only; raises ``OutOfRangeError`` at the end of an epoch."""
-        if self._q_iter is None:
-            from ..gsl.iterators import SeedIterator
-            self._q_vids = self.csr.insertion_pos().cpu()
-            self._q_iter = SeedIterator(int(self._q_vids.numel()), self.batch_size, "shuffle", "cpu",
-                                        seed=_config.get().seed + 17 * self.rt.rank, drop_last=True)
-            self._q_epoch, self._q_order = -1, None
+        if self._q_iter is None:        # the traversal hands CSR positions to ``_fill_slot``
+            self._set_traversal(self.csr.insertion_pos().cpu(), self.batch_size, "shuffle")
         return self.step_query()
-
-    def _q_step(self, pos: torch.Tensor) -> torch.Tensor:
-        return self._step_staged(pos, None)
 
     def step_device(self, next_src: Optional[torch.Tensor] = None, next_dst: Optional[torch.Tensor] = None):
         """Device-only step.  ``next_src`` / ``next_dst`` (device int64 [B] vids) are the edges of the batch the replay
         samples for the FOLLOWING step; without them the resident edges get fresh negatives and hops."""
-        if next_src is not None:
-            B = self.batch_size
-            if self.graph is None:
-                bufs = [self.seeds]
-            else:
-                i = self._steps & 1
-                bufs = [self._hops[i ^ 1][0]] + ([] if self._primed else [self._hops[i][0]])
-            for r in bufs:
-                self.C.copy_i64(r[:B], next_src)
-                self.C.copy_i64(r[B:2 * B], next_dst)
-        FastSageTrainer.step_device(self)
+        self._step_device(next_src, next_dst)
 
     @torch.no_grad()
     def embed(self, vids: torch.Tensor) -> torch.Tensor:

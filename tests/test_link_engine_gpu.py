@@ -229,6 +229,36 @@ def test_link_engine_e2e_pipeline_staging(rt):
     assert torch.equal(roots(tr2.seeds), torch.cat(e[3])) and float(l) > 0
 
 
+@pytest.mark.parametrize("link", [False, True], ids=["supervised", "link"])
+def test_eager_step_trains_on_its_own_batch_when_host_runs_ahead(rt, link):
+    """Without CUDA graphs, step() refills pinned staging memory on the host.  When the host runs ahead of the GPU,
+    a later call must not overwrite a batch that the device has not read yet: step t trains on the roots of call t."""
+    from graphlearn_b200.engine import FastLinkSageTrainer, FastSageTrainer
+    from graphlearn_b200.models.graphsage import EgoGraphSAGE
+    from graphlearn_b200.store.synthetic import make_sharded_graph
+    nodes, csr = make_sharded_graph(rt, 20000, 400000, 64, 8, seed=11)
+    B = 128
+    if link:
+        tr = FastLinkSageTrainer(rt, nodes, csr, EgoGraphSAGE(64, 128, 32, 2).to(rt.device), [5, 4], B, 3,
+                                 use_cuda_graph=False)
+        batches = [(torch.randint(0, 20000, (B,)), torch.randint(0, 20000, (B,))) for _ in range(4)]
+    else:
+        tr = FastSageTrainer(rt, nodes, csr, EgoGraphSAGE(64, 128, 8, 2).to(rt.device), [5, 4], B,
+                             use_cuda_graph=False)
+        batches = [(torch.randint(0, 20000, (B,)),) for _ in range(4)]
+    tr.step(*batches[0]); torch.cuda.synchronize()        # first launches load their modules
+    want = [torch.cat(b) for b in batches[1:3]]
+    snaps = [torch.empty_like(w, device=rt.device) for w in want]
+    torch.cuda._sleep(400_000_000)                         # ~0.2 s at 1.98 GHz: the GPU lags the host
+    for b, snap in zip(batches[1:3], snaps):
+        tr.step(*b)
+        snap.copy_(tr.seeds[:snap.numel()])                # the roots this step trained on
+    tr.step(*batches[3])                                   # reuses the staging memory of batches[1]
+    torch.cuda.synchronize()
+    for snap, w in zip(snaps, want):
+        assert torch.equal(snap.cpu(), w)
+
+
 # ------------------------------------------------------------------------------------- 6. edge traversal epochs
 def test_link_engine_step_edges_epochs(rt):
     from graphlearn_b200 import errors
