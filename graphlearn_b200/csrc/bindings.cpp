@@ -37,6 +37,9 @@ void sage_fused_multi(const at::Tensor&, const at::Tensor&, const std::vector<c1
                       const std::vector<c10::optional<at::Tensor>>&, int64_t, const at::Tensor&,
                       const c10::optional<at::Tensor>&, int64_t, int64_t, bool, bool,
                       const std::vector<c10::optional<at::Tensor>>&, int64_t, int64_t, int64_t);
+void sage_fused_csr(const at::Tensor&, const at::Tensor&, const at::Tensor&, const at::Tensor&, const at::Tensor&,
+                    const std::vector<at::Tensor>&, const at::Tensor&, int64_t, const at::Tensor&,
+                    const c10::optional<at::Tensor>&, int64_t, int64_t, bool, bool, int64_t, int64_t);
 int sm_count();
 void sage_set_debug_trace(const c10::optional<at::Tensor>&);
 // sage_bwd.cu
@@ -174,6 +177,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("sage_smem_bytes", &glb::sage_smem_bytes);
   m.def("sage_fused_forward", &glb::sage_fused_forward);
   m.def("sage_fused_multi", &glb::sage_fused_multi);
+  m.def("sage_fused_csr", &glb::sage_fused_csr);
   m.def("sm_count", &glb::sm_count);
   m.def("sage_set_debug_trace", &glb::sage_set_debug_trace);
   m.def("pack_weight_t", &glb::pack_weight_t);

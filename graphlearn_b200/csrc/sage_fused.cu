@@ -99,6 +99,15 @@ struct SageParams {
   // b / n_imgs + j * (gridDim.x / n_imgs) and writes output columns [img * N, img * N + n_out)
   int n_imgs;
   long long* dbg;             // optional [grid][64] clock64 trace (tools/persist_timeline.py), lane 0 of one warp per role
+  // CSR neighbour mode (sage_persist_kernel<U, DT, true>, one segment): the neighbours of destination row m are the vids
+  // csr_indices[csr_indptr[m] .. csr_indptr[m + 1]); rows with hub_map[m] = h >= 0 instead sum the fp32 partial rows
+  // hub_part[hub_cptr[h] .. hub_cptr[h + 1]) of sage_hub_partial_kernel (row stride hub_stride = kp_nbr floats)
+  const int64_t* csr_indptr;
+  const int64_t* csr_indices;
+  const int* hub_map;
+  const int* hub_cptr;
+  const float* hub_part;
+  int hub_stride;
 };
 
 // write VEC consecutive K elements of tile row r starting at K column kcol (multiple of VEC)
@@ -287,15 +296,235 @@ __device__ __forceinline__ void write_item_ptrs(const SageParams& p, const TileC
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// CSR neighbour mode (layer-wise full-neighbourhood inference): the neighbours of destination row m are the CSR row
+// csr_indices[csr_indptr[m] .. csr_indptr[m + 1]) of any length.  An item is ONE destination row x one 512-byte slice:
+// the warp's 32 / lpr lane groups split the row's neighbours (group g takes every ngrp-th one) and are summed with
+// shuffles at the end, so a warp's time follows the degree of its own row, not the largest of several packed rows.  The
+// adjacency is walked in rounds of kScrCap ids: ids -> row pointers (vid_ptr) in the warp's scratch -> U-batched row
+// loads.  The id range of the NEXT item is prefetched at the top of an item and its first round of ids right after
+// the current row loads.  Hub rows (hub_map >= 0) sum the fp32 partial rows of their adjacency chunks instead.
+// ------------------------------------------------------------------------------------------------
+template <int U, int DT>
+__device__ __forceinline__ void sage_csr_gather(const SageParams& p, uint8_t* sA, uint32_t a_buf_bytes, uint64_t* bars,
+                                                const char** scr, int tile_first, int tile_stride, int gw, int lane) {
+  constexpr int VEC = Chunk<DT>::kVec;
+  constexpr uint32_t kEsz = DT == 0 ? 4u : DT == 1 ? 2u : 1u;
+  const SageSeg& sg = p.seg[0];
+  const int kp = p.kp_nbr > 0 ? p.kp_nbr : p.kp_self;
+  const int d_self = p.tself.dim, d_nbr = p.tnbr.dim;
+  const int lanes_row = kp / VEC;
+  const int lpr = lanes_row < 32 ? lanes_row : 32;
+  const int ngrp = 32 / lpr;                            // lane groups sharing the destination row
+  const int grp = lane / lpr;
+  GatherGeom gg;                                        // one destination row per item
+  gg.lshift = 5; gg.rpi = 1; gg.sub = 0;
+  gg.n_slices = lanes_row > 32 ? lanes_row >> 5 : 1;
+  gg.lig = lane & (lpr - 1);
+  gg.tile_first = tile_first; gg.tile_stride = tile_stride;
+  const bool has_self = p.kp_self > 0, has_nbr = p.kp_nbr > 0;
+  const uint32_t nbr_row_bytes = (uint32_t)p.tnbr.stride * kEsz, self_row_bytes = (uint32_t)p.tself.stride * kEsz;
+  const int soff_self = fp8_scale_offset(d_self), soff_nbr = fp8_scale_offset(d_nbr);
+  const int n_tiles_cta = (p.total_tiles - tile_first + tile_stride - 1) / tile_stride;
+
+  int arrived = 0;                                      // as in the sampled gather role
+  auto arrive_upto = [&](int upto) {
+    while (arrived < upto) {
+      gmma::mbar_wait(bars + kBarAFree + (arrived & 1), (uint32_t)(((arrived >> 1) & 1) ^ 1));
+      if (lane == 0) gmma::mbar_arrive(bars + kBarAFull + (arrived & 1));
+      ++arrived;
+    }
+  };
+  auto fetch_ids = [&](int64_t e0, int64_t e1, int64_t (&v)[2]) {
+#pragma unroll
+    for (int u = 0; u < 2; ++u) v[u] = e0 + lane + 32 * u < e1 ? __ldg(p.csr_indices + e0 + lane + 32 * u) : -1;
+  };
+
+  int it = 0, item = gw;
+  TileCtx cur;
+  bool valid = seek_item(p, gg, it, item, cur);
+  int64_t e_beg = 0, e_end = 0;
+  int hub = -1;
+  int64_t ids[2] = {-1, -1};                            // first round of ids of the current item
+  if (valid) {
+    const int m = cur.m0 + (gg.n_slices == 1 ? item : item / gg.n_slices);
+    e_beg = __ldg(p.csr_indptr + m); e_end = __ldg(p.csr_indptr + m + 1);
+    hub = p.hub_map ? __ldg(p.hub_map + m) : -1;
+    if (has_nbr && hub < 0) fetch_ids(e_beg, e_end, ids);
+  }
+  while (valid) {
+    int nit = it, nitem = item + kGatherWarps;
+    TileCtx nxt;
+    const bool nvalid = seek_item(p, gg, nit, nitem, nxt);
+    int64_t nb = 0, ne = 0;
+    int nhub = -1;
+    if (nvalid) {
+      const int nm = nxt.m0 + (gg.n_slices == 1 ? nitem : nitem / gg.n_slices);
+      nb = __ldg(p.csr_indptr + nm); ne = __ldg(p.csr_indptr + nm + 1);
+      nhub = p.hub_map ? __ldg(p.hub_map + nm) : -1;
+    }
+    const int rg = gg.n_slices == 1 ? item : item / gg.n_slices;      // row of the tile
+    const int sl = gg.n_slices == 1 ? 0 : item - rg * gg.n_slices;
+    const int m = cur.m0 + rg;
+    const int chunk = gg.lig + 32 * sl;
+    const int f0 = chunk * VEC;
+    float acc[VEC], sv[VEC];
+#pragma unroll
+    for (int i = 0; i < VEC; ++i) { acc[i] = 0.f; sv[i] = 0.f; }
+    const bool self_ld = has_self && grp == 0 && f0 < d_self;
+    Chunk<DT> sraw;
+    if (self_ld)
+      load_chunk<DT>(sraw, vid_ptr(p.tself, sg.self_vids ? __ldg(sg.self_vids + m) : sg.self_base + m, p.wshift_self,
+                                   self_row_bytes, p.zero_row), chunk, soff_self);
+    if (has_nbr && hub >= 0) {
+      if (f0 < d_nbr) {
+        const int c1 = __ldg(p.hub_cptr + hub + 1);
+        for (int c = __ldg(p.hub_cptr + hub) + grp; c < c1; c += ngrp) {
+          const float4* src = reinterpret_cast<const float4*>(p.hub_part + (size_t)c * p.hub_stride + f0);
+#pragma unroll
+          for (int q = 0; q < VEC / 4; ++q) {
+            const float4 v = __ldcg(src + q);
+            acc[4 * q] += v.x; acc[4 * q + 1] += v.y; acc[4 * q + 2] += v.z; acc[4 * q + 3] += v.w;
+          }
+        }
+      }
+    } else if (has_nbr) {
+      for (int64_t e0 = e_beg; e0 < e_end; e0 += kScrCap) {
+        if (e0 != e_beg) fetch_ids(e0, e_end, ids);
+        const int n = (int)(e_end - e0 < kScrCap ? e_end - e0 : kScrCap);
+        __syncwarp();                                   // every lane is done reading the previous round's pointers
+#pragma unroll
+        for (int u = 0; u < 2; ++u)
+          if (lane + 32 * u < n) scr[lane + 32 * u] = vid_ptr(p.tnbr, ids[u], p.wshift_nbr, nbr_row_bytes, p.zero_row);
+        __syncwarp();
+        if (f0 < d_nbr) {
+          int j = grp;
+          for (; j + (U - 1) * ngrp < n; j += U * ngrp) {
+            Chunk<DT> raw[U];
+#pragma unroll
+            for (int u = 0; u < U; ++u) load_chunk<DT>(raw[u], scr[j + u * ngrp], chunk, soff_nbr);
+#pragma unroll
+            for (int u = 0; u < U; ++u) raw[u].add_to(acc);
+          }
+          if (j < n) {
+            Chunk<DT> raw[U];
+#pragma unroll
+            for (int u = 0; u < U; ++u) load_chunk<DT>(raw[u], scr[j + u * ngrp < n ? j + u * ngrp : j], chunk, soff_nbr);
+#pragma unroll
+            for (int u = 0; u < U; ++u)
+              if (j + u * ngrp < n) raw[u].add_to(acc);
+          }
+        }
+      }
+    }
+    if (nvalid && has_nbr && nhub < 0) fetch_ids(nb, ne, ids);
+#pragma unroll
+    for (int o = lpr; o < 32; o <<= 1)                  // sum the lane groups' shares of the row
+#pragma unroll
+      for (int i = 0; i < VEC; ++i) acc[i] += __shfl_xor_sync(0xffffffffu, acc[i], o);
+    if (self_ld) sraw.add_to(sv);
+    if (f0 + VEC > d_self || f0 + VEC > d_nbr) {
+#pragma unroll
+      for (int i = 0; i < VEC; ++i) {
+        if (f0 + i >= d_self) sv[i] = 0.f;
+        if (f0 + i >= d_nbr) acc[i] = 0.f;
+      }
+    }
+    arrive_upto(it);
+    gmma::mbar_wait(bars + kBarAFree + (it & 1), (uint32_t)(((it >> 1) & 1) ^ 1));
+    uint8_t* sAt = sA + (size_t)(it & 1) * a_buf_bytes;
+    if (grp == 0) {
+      if (has_self) put_chunk<VEC>(sAt, nullptr, rg, f0, sv);
+      if (has_nbr) {
+        const int64_t deg = e_end - e_beg;              // degree 0: zero aggregate
+        const float scale = p.mode == kConcatMean ? (deg > 0 ? 1.f / (float)deg : 0.f) : 1.f;
+#pragma unroll
+        for (int i = 0; i < VEC; ++i) acc[i] *= scale;
+        put_chunk<VEC>(sAt, nullptr, rg, p.kp_self + f0, acc);
+      }
+    }
+    if (!nvalid || nit != it) {                         // last item of this warp in tile `it`
+      gmma::fence_proxy_async_smem();
+      __syncwarp();
+      if (lane == 0) gmma::mbar_arrive(bars + kBarAFull + (it & 1));
+      arrived = it + 1;
+    }
+    it = nit; item = nitem; cur = nxt; valid = nvalid;
+    e_beg = nb; e_end = ne; hub = nhub;
+  }
+  arrive_upto(n_tiles_cta);
+}
+
+// Hub pre-pass of the CSR mode.  The host cuts the adjacency of every row above its hub degree into chunks of a few
+// hundred edges (static per CSR); one warp per (chunk, 512-byte slice) sums the chunk's neighbour rows in fp32 into
+// part[chunk, 0 .. kp).  The layer launch then reads a hub row's few partial rows instead of its neighbours, so a row of
+// 50 000 neighbours is spread over hundreds of warps instead of stalling one gather warp - and with it, through the
+// double-buffered A tile, its whole CTA.  Fixed chunking and summation order: the result is deterministic.
+template <int U, int DT>
+__global__ void __launch_bounds__(256) sage_hub_partial_kernel(const __grid_constant__ TableView t, int wshift, const int64_t* __restrict__ indices,
+                                                               const int64_t* __restrict__ chunks, int n_chunks, int kp,
+                                                               float* __restrict__ part, const char* zero_row) {
+  constexpr int VEC = Chunk<DT>::kVec;
+  constexpr uint32_t kEsz = DT == 0 ? 4u : DT == 1 ? 2u : 1u;
+  const int lanes_row = kp / VEC;
+  const int lpr = lanes_row < 32 ? lanes_row : 32;
+  const int ngrp = 32 / lpr;
+  const int n_slices = lanes_row > 32 ? lanes_row >> 5 : 1;
+  const int lane = threadIdx.x & 31;
+  const int w = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+  if (w >= n_chunks * n_slices) return;                // whole warps
+  const int c = w / n_slices, sl = w - c * n_slices;
+  const int grp = lane / lpr;
+  const int chunk = (lane & (lpr - 1)) + 32 * sl;
+  const int f0 = chunk * VEC;
+  const int64_t e0 = __ldg(chunks + 2 * c);
+  const int64_t* ids = indices + e0;
+  const int cnt = (int)(__ldg(chunks + 2 * c + 1) - e0);   // <= the host's chunk size
+  const uint32_t row_bytes = (uint32_t)t.stride * kEsz;
+  const int soff = fp8_scale_offset(t.dim);
+  float acc[VEC];
+#pragma unroll
+  for (int i = 0; i < VEC; ++i) acc[i] = 0.f;
+  if (f0 < t.dim) {
+    for (int j = grp; j < cnt; j += U * ngrp) {
+      const char* ptr[U];
+#pragma unroll
+      for (int u = 0; u < U; ++u) {
+        const int ju = j + u * ngrp;
+        ptr[u] = ju < cnt ? vid_ptr(t, __ldg(ids + ju), wshift, row_bytes, zero_row) : zero_row;
+      }
+      Chunk<DT> raw[U];
+#pragma unroll
+      for (int u = 0; u < U; ++u) load_chunk<DT>(raw[u], ptr[u], chunk, soff);
+#pragma unroll
+      for (int u = 0; u < U; ++u) raw[u].add_to(acc);
+    }
+  }
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    if (o < lpr) continue;                              // (warp-uniform)
+#pragma unroll
+    for (int i = 0; i < VEC; ++i) acc[i] += __shfl_xor_sync(0xffffffffu, acc[i], o);
+  }
+  if (grp == 0) {
+    float4* dst = reinterpret_cast<float4*>(part + (size_t)c * kp + f0);
+#pragma unroll
+    for (int q = 0; q < VEC / 4; ++q)
+      dst[q] = make_float4(f0 + 4 * q < t.dim ? acc[4 * q] : 0.f, f0 + 4 * q + 1 < t.dim ? acc[4 * q + 1] : 0.f,
+                           f0 + 4 * q + 2 < t.dim ? acc[4 * q + 2] : 0.f, f0 + 4 * q + 3 < t.dim ? acc[4 * q + 3] : 0.f);
+  }
+}
+
 // U  = neighbour row loads kept in flight per lane (one batch)
 // DT = storage dtype of the self AND neighbour tables (0 fp32, 1 bf16)
+// CSR = neighbour source: fixed-k id lists of the segments (false) or CSR rows of any length (true, sage_csr_gather)
 //
 // Gather decomposition: a row needs LPR = kp / VEC lanes (16-byte chunk per lane); when LPR < 32 a
 // warp processes 32/LPR rows side by side (sub-warp groups), when LPR > 32 the row is cut into
 // 32-lane slices.  Per item a lane group issues ALL self + neighbour chunk loads of a batch
 // unconditionally (masked lanes read a zero row), reduces in fp32 and writes bf16 into the SW128
 // A tile.
-template <int U, int DT>
+template <int U, int DT, bool CSR = false>
 __global__ void __launch_bounds__(kThreads, 1) sage_persist_kernel(const __grid_constant__ SageParams p) {
   if (p.dbg && threadIdx.x == 0) {
     unsigned long long gt; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt));
@@ -390,6 +619,9 @@ __global__ void __launch_bounds__(kThreads, 1) sage_persist_kernel(const __grid_
     __syncwarp();
     gmma::mbar_wait(bars + kBarW, 0);
     GLB_DBG(1);
+  } else if constexpr (CSR) {
+    sage_csr_gather<U, DT>(p, sA, a_buf_bytes, bars, sScr + (warp - kGatherWarp0) * kScrCap, tile_first, tile_stride,
+                           warp - kGatherWarp0, lane);
   } else {
     // =================================================================== gather warps
     constexpr int VEC = Chunk<DT>::kVec;
@@ -641,27 +873,84 @@ static void plan_tiles(SageParams& p, int usable_sms) {
   p.total_tiles = tiles;
 }
 
-static void launch_persist(SageParams& p, size_t smem, int usable_sms, cudaStream_t stream) {
+template <int U, int DT, bool CSR>
+static void launch_one(const SageParams& p, unsigned grid, size_t smem, cudaStream_t stream) {
+  static bool attr_done = false;
+  if (!attr_done) {
+    C10_CUDA_CHECK(cudaFuncSetAttribute(sage_persist_kernel<U, DT, CSR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemLimit));
+    attr_done = true;
+  }
+  sage_persist_kernel<U, DT, CSR><<<grid, kThreads, smem, stream>>>(p);
+}
+
+// row loads in flight per lane of the CSR mode (one instantiation per table dtype)
+constexpr int kCsrU = 5;
+
+static void launch_persist(SageParams& p, size_t smem, int usable_sms, cudaStream_t stream, bool csr = false) {
   if (p.total_tiles == 0) return;
   const unsigned grid = (unsigned)(p.n_imgs * std::min<int>(std::max(1, usable_sms / p.n_imgs), p.total_tiles));
   int kmax = 1;
   for (int s = 0; s < p.nseg; ++s) kmax = std::max(kmax, p.seg[s].k);
   const int dt = p.tnbr.dtype;
-#define LAUNCH(UU, DD)                                                                                     \
-  do {                                                                                                     \
-    static bool attr_done = false;                                                                         \
-    if (!attr_done) {                                                                                      \
-      C10_CUDA_CHECK(cudaFuncSetAttribute(sage_persist_kernel<UU, DD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemLimit)); \
-      attr_done = true;                                                                                    \
-    }                                                                                                      \
-    sage_persist_kernel<UU, DD><<<grid, kThreads, smem, stream>>>(p);                                      \
-  } while (0)
-#define LAUNCH_DT3(UU) do { if (dt == 2) LAUNCH(UU, 2); else if (dt == 0) LAUNCH(UU, 0); else LAUNCH(UU, 1); } while (0)
+#define LAUNCH_DT3(UU, CC) do { if (dt == 2) launch_one<UU, 2, CC>(p, grid, smem, stream); \
+                                else if (dt == 0) launch_one<UU, 0, CC>(p, grid, smem, stream); \
+                                else launch_one<UU, 1, CC>(p, grid, smem, stream); } while (0)
   const int u = kmax <= 4 ? 4 : (kmax % 5 == 0 || kmax > 12) ? 5 : 6;
-  if (u == 4) LAUNCH_DT3(4); else if (u == 5) LAUNCH_DT3(5); else LAUNCH_DT3(6);
+  if (csr) LAUNCH_DT3(kCsrU, true);
+  else if (u == 4) LAUNCH_DT3(4, false); else if (u == 5) LAUNCH_DT3(5, false); else LAUNCH_DT3(6, false);
 #undef LAUNCH_DT3
-#undef LAUNCH
   C10_CUDA_KERNEL_LAUNCH_CHECK();
+}
+
+// Launch-wide fields and checks shared by both entry points: tables, padded K, weight image, bias, output format.
+// Returns the dynamic shared memory of the launch; `b` keeps a contiguous copy of the bias alive.
+static size_t init_layer_params(SageParams& p, const at::Tensor& tself_desc, const at::Tensor& tnbr_desc, bool any_nbr, int64_t mode,
+                                const at::Tensor& w_img, const c10::optional<at::Tensor>& bias, at::Tensor& b, int64_t N,
+                                int64_t n_out, bool relu, bool out_bf16, int64_t n_imgs) {
+  std::memset(&p, 0, sizeof(p));
+  p.tself = table_from_desc(tself_desc);
+  p.tnbr = table_from_desc(tnbr_desc);
+  p.mode = (int)mode;
+  p.kp_self = (mode == kGcnMean) ? 0 : pad_k(p.tself.dim);
+  p.kp_nbr = any_nbr ? pad_k(p.tnbr.dim) : 0;
+  if (mode == kGcnMean) TORCH_CHECK(p.tself.dim == p.tnbr.dim, "gcn mode needs equal dims");
+  const int k_total = p.kp_self + p.kp_nbr;
+  TORCH_CHECK(k_total >= 64, "empty layer");
+  TORCH_CHECK(N % 32 == 0 && N >= 32 && N <= 256, "padded N must be a multiple of 32 in [32, 256]");
+  TORCH_CHECK(n_out <= N && n_out >= 1);
+  TORCH_CHECK(n_imgs >= 1 && n_imgs <= 8 && (n_imgs == 1 || n_out == N), "bad image count");
+  p.n_imgs = (int)n_imgs;
+  TORCH_CHECK(w_img.numel() == n_imgs * (int64_t)k_total * N, "weight image size mismatch: expected ", n_imgs * k_total * N, " got ", w_img.numel());
+  TORCH_CHECK((reinterpret_cast<uintptr_t>(w_img.data_ptr()) & 15) == 0, "weight image must be 16 B aligned");
+  const size_t smem = (size_t)sage_smem_bytes(k_total, N);
+  TORCH_CHECK(smem <= kSmemLimit, "tile does not fit in shared memory (", smem, " B); use the unfused path");
+  TORCH_CHECK(p.tself.dtype == p.tnbr.dtype, "fused SAGE layer needs self / neighbour tables of the same storage dtype");
+  TORCH_CHECK(p.kp_self == 0 || p.kp_nbr == 0 || p.kp_self == p.kp_nbr, "fused SAGE layer needs equally padded self / neighbour dims");
+  TORCH_CHECK((p.tself.stride * table_esize(p.tself.dtype)) % 16 == 0 && (p.tnbr.stride * table_esize(p.tnbr.dtype)) % 16 == 0,
+              "table rows must be 16-byte aligned (stride multiple of 4 fp32 / 8 bf16 elements)");
+  if (bias.has_value() && bias->defined()) {
+    b = bias->contiguous();
+    TORCH_CHECK(b.is_cuda() && b.scalar_type() == at::kFloat && (n_imgs > 1 || b.numel() >= n_out), "bias must be fp32 [>= n_out]");
+    p.bias = b.data_ptr<float>();
+    p.bias_len = (int)b.numel();
+  }
+  p.w_img = w_img.data_ptr();
+  p.N = (int)N; p.n_out = (int)n_out; p.relu = relu ? 1 : 0; p.out_bf16 = out_bf16 ? 1 : 0;
+  p.wshift_self = log2_or_neg(p.tself.world);
+  p.wshift_nbr = log2_or_neg(p.tnbr.world);
+  p.zero_row = zero_row_for(w_img.options(), w_img.get_device());
+  return smem;
+}
+
+// output rows of one segment (an undefined tensor: no output); every segment of a launch shares the row stride
+static void set_seg_out(SageParams& p, SageSeg& sg, const at::Tensor& out, int64_t M, int64_t n_out, bool out_bf16) {
+  if (!out.defined()) return;
+  TORCH_CHECK(out.is_cuda() && out.dim() == 2 && out.size(0) == M && out.size(1) == n_out && out.stride(1) == 1,
+              "outs[i] must be [M_i, n_out] with unit inner stride");
+  TORCH_CHECK(out.scalar_type() == (out_bf16 ? at::kBFloat16 : at::kFloat), "out dtype mismatch");
+  TORCH_CHECK(p.out_stride < 0 || p.out_stride == out.stride(0), "all outputs must share the row stride");
+  p.out_stride = out.stride(0);
+  sg.out = reinterpret_cast<char*>(out.data_ptr());
 }
 
 // Multi-segment entry point.  All segments share the tables, the weight image, the bias and the output
@@ -688,30 +977,11 @@ void sage_fused_multi(const at::Tensor& tself_desc, const at::Tensor& tnbr_desc,
               (int)self_vids.size() == nseg && (int)nbr_vids.size() == nseg && (int)self_base.size() == nseg &&
               (int)nbr_base.size() == nseg, "per-segment argument lists must have equal lengths");
   SageParams p;
-  std::memset(&p, 0, sizeof(p));
-  p.tself = table_from_desc(tself_desc);
-  p.tnbr = table_from_desc(tnbr_desc);
-  p.nseg = nseg;
-  p.mode = (int)mode;
   bool any_nbr = false;
   for (int s = 0; s < nseg; ++s) any_nbr = any_nbr || ks[s] > 0;
-  p.kp_self = (mode == kGcnMean) ? 0 : pad_k(p.tself.dim);
-  p.kp_nbr = any_nbr ? pad_k(p.tnbr.dim) : 0;
-  if (mode == kGcnMean) TORCH_CHECK(p.tself.dim == p.tnbr.dim, "gcn mode needs equal dims");
-  const int k_total = p.kp_self + p.kp_nbr;
-  TORCH_CHECK(k_total >= 64, "empty layer");
-  TORCH_CHECK(N % 32 == 0 && N >= 32 && N <= 256, "padded N must be a multiple of 32 in [32, 256]");
-  TORCH_CHECK(n_out <= N && n_out >= 1);
-  TORCH_CHECK(n_imgs >= 1 && n_imgs <= 8 && (n_imgs == 1 || n_out == N), "bad image count");
-  p.n_imgs = (int)n_imgs;
-  TORCH_CHECK(w_img.numel() == n_imgs * (int64_t)k_total * N, "weight image size mismatch: expected ", n_imgs * k_total * N, " got ", w_img.numel());
-  TORCH_CHECK((reinterpret_cast<uintptr_t>(w_img.data_ptr()) & 15) == 0, "weight image must be 16 B aligned");
-  const size_t smem = (size_t)sage_smem_bytes(k_total, N);
-  TORCH_CHECK(smem <= kSmemLimit, "tile does not fit in shared memory (", smem, " B); use the unfused path");
-  TORCH_CHECK(p.tself.dtype == p.tnbr.dtype, "fused SAGE layer needs self / neighbour tables of the same storage dtype");
-  TORCH_CHECK(p.kp_self == 0 || p.kp_nbr == 0 || p.kp_self == p.kp_nbr, "fused SAGE layer needs equally padded self / neighbour dims");
-  TORCH_CHECK((p.tself.stride * table_esize(p.tself.dtype)) % 16 == 0 && (p.tnbr.stride * table_esize(p.tnbr.dtype)) % 16 == 0,
-              "table rows must be 16-byte aligned (stride multiple of 4 fp32 / 8 bf16 elements)");
+  at::Tensor b;
+  const size_t smem = init_layer_params(p, tself_desc, tnbr_desc, any_nbr, mode, w_img, bias, b, N, n_out, relu, out_bf16, n_imgs);
+  p.nseg = nseg;
   {
     const int vec = p.tnbr.dtype == 0 ? 4 : 8;
     const int lanes_row = (p.kp_nbr > 0 ? p.kp_nbr : p.kp_self) / vec;
@@ -720,13 +990,7 @@ void sage_fused_multi(const at::Tensor& tself_desc, const at::Tensor& tnbr_desc,
       TORCH_CHECK(rpi * (ks[s] + 1) <= kScrCap, "fan-out too large for the fused kernel's pointer scratch: k <= ", kScrCap / rpi - 1);
   }
   std::vector<at::Tensor> keep;
-  at::Tensor b;
-  if (bias.has_value() && bias->defined()) {
-    b = bias->contiguous();
-    TORCH_CHECK(b.is_cuda() && b.scalar_type() == at::kFloat && (n_imgs > 1 || b.numel() >= n_out), "bias must be fp32 [>= n_out]");
-    p.bias = b.data_ptr<float>();
-    p.bias_len = (int)b.numel();
-  }
+  const int k_total = p.kp_self + p.kp_nbr;
   p.out_stride = -1;
   for (int s = 0; s < nseg; ++s) {
     SageSeg& sg = p.seg[s];
@@ -740,15 +1004,7 @@ void sage_fused_multi(const at::Tensor& tself_desc, const at::Tensor& tnbr_desc,
       at::Tensor t = nbr_vids[s]->contiguous(); check_cuda_i64(t, "nbr_vids");
       TORCH_CHECK(t.numel() == Ms[s] * ks[s]); keep.push_back(t); sg.nbr_vids = t.data_ptr<int64_t>();
     }
-    const at::Tensor& out = outs[s];
-    if (out.defined()) {
-      TORCH_CHECK(out.is_cuda() && out.dim() == 2 && out.size(0) == Ms[s] && out.size(1) == n_out && out.stride(1) == 1,
-                  "outs[i] must be [M_i, n_out] with unit inner stride");
-      TORCH_CHECK(out.scalar_type() == (out_bf16 ? at::kBFloat16 : at::kFloat), "out dtype mismatch");
-      TORCH_CHECK(p.out_stride < 0 || p.out_stride == out.stride(0), "all outputs must share the row stride");
-      p.out_stride = out.stride(0);
-      sg.out = reinterpret_cast<char*>(out.data_ptr());
-    }
+    set_seg_out(p, sg, outs[s], Ms[s], n_out, out_bf16);
     if (a_saves[s].has_value() && a_saves[s]->defined()) {
       const at::Tensor& a = *a_saves[s];
       TORCH_CHECK(a.scalar_type() == at::kBFloat16 && a.dim() == 2 && a.size(0) == Ms[s] && a.size(1) == k_total &&
@@ -757,11 +1013,6 @@ void sage_fused_multi(const at::Tensor& tself_desc, const at::Tensor& tnbr_desc,
     }
   }
   if (p.out_stride < 0) p.out_stride = n_out;
-  p.w_img = w_img.data_ptr();
-  p.N = (int)N; p.n_out = (int)n_out; p.relu = relu ? 1 : 0; p.out_bf16 = out_bf16 ? 1 : 0;
-  p.wshift_self = log2_or_neg(p.tself.world);
-  p.wshift_nbr = log2_or_neg(p.tnbr.world);
-  p.zero_row = zero_row_for(w_img.options(), w_img.get_device());
   if (!ce.empty()) {
     TORCH_CHECK(ce.size() == 5 && nseg == 1 && N <= 64, "fused CE needs one segment and n_out <= 64");
     TORCH_CHECK(p.seg[0].out != nullptr && !out_bf16, "fused CE needs the fp32 logits output (its second phase re-reads it)");
@@ -793,6 +1044,76 @@ void sage_fused_multi(const at::Tensor& tself_desc, const at::Tensor& tnbr_desc,
   const int usable_sms = max_ctas > 0 ? std::min<int>(sm_count(), (int)max_ctas) : sm_count();
   plan_tiles(p, usable_sms);
   launch_persist(p, smem, usable_sms, at::cuda::getCurrentCUDAStream());
+}
+
+// Layer-wise full-neighbourhood inference: ONE layer over every row of a CSR (row m of `out` aggregates the neighbour
+// rows csr_indices[csr_indptr[m] .. csr_indptr[m + 1]) of tnbr; its self row is self_vids[m] in tself).
+// hubs = [] or [hub_map int32 [M] (-1 = ordinary row), hub_cptr int32 [n_hub + 1], chunks int64 [n_chunks, 2]
+// (edge ranges), part fp32 [>= n_chunks * kp_nbr]]: the hub rows' adjacency chunks are first summed into `part` by
+// sage_hub_partial_kernel.  plan_deg = mean degree of the ordinary rows (tile costing).
+void sage_fused_csr(const at::Tensor& tself_desc, const at::Tensor& tnbr_desc, const at::Tensor& self_vids,
+                    const at::Tensor& csr_indptr, const at::Tensor& csr_indices, const std::vector<at::Tensor>& hubs,
+                    const at::Tensor& out, int64_t mode, const at::Tensor& w_img, const c10::optional<at::Tensor>& bias,
+                    int64_t N, int64_t n_out, bool relu, bool out_bf16, int64_t n_imgs, int64_t plan_deg) {
+  TORCH_CHECK(w_img.is_cuda() && w_img.scalar_type() == at::kBFloat16, "w_img must be CUDA bf16");
+  c10::cuda::CUDAGuard guard(w_img.device());
+  TORCH_CHECK(mode == kConcatMean || mode == kConcatSum, "CSR mode supports mean / sum aggregation");
+  const int64_t M = self_vids.numel();
+  check_cuda_i64(self_vids, "self_vids");
+  check_cuda_i64(csr_indptr, "csr_indptr");
+  check_cuda_i64(csr_indices, "csr_indices");
+  TORCH_CHECK(self_vids.is_contiguous() && csr_indptr.is_contiguous() && csr_indices.is_contiguous(), "CSR operands must be contiguous");
+  TORCH_CHECK(csr_indptr.numel() == M + 1, "csr_indptr must have M + 1 entries");
+  TORCH_CHECK(M < (int64_t)INT32_MAX, "too many rows");
+  SageParams p;
+  at::Tensor b;
+  const size_t smem = init_layer_params(p, tself_desc, tnbr_desc, true, mode, w_img, bias, b, N, n_out, relu, out_bf16, n_imgs);
+  p.nseg = 1;
+  SageSeg& sg = p.seg[0];
+  sg.M = (int)M;
+  sg.k = (int)std::max<int64_t>(plan_deg, 1);        // tile costing only: the CSR gather reads the row's own degree
+  sg.self_vids = self_vids.data_ptr<int64_t>();
+  p.out_stride = -1;
+  set_seg_out(p, sg, out, M, n_out, out_bf16);
+  TORCH_CHECK(sg.out != nullptr, "CSR mode needs an output");
+  p.csr_indptr = csr_indptr.data_ptr<int64_t>();
+  p.csr_indices = csr_indices.data_ptr<int64_t>();
+  const cudaStream_t stream = at::cuda::getCurrentCUDAStream();
+  if (!hubs.empty()) {
+    TORCH_CHECK(hubs.size() == 4, "hubs = [hub_map, hub_cptr, chunks, part]");
+    const at::Tensor &hmap = hubs[0], &cptr = hubs[1], &chunks = hubs[2], &part = hubs[3];
+    TORCH_CHECK(hmap.is_cuda() && hmap.scalar_type() == at::kInt && hmap.numel() == M && hmap.is_contiguous(), "hub_map must be int32 [M]");
+    TORCH_CHECK(cptr.is_cuda() && cptr.scalar_type() == at::kInt && cptr.is_contiguous() && cptr.numel() >= 1, "hub_cptr must be int32");
+    check_cuda_i64(chunks, "chunks");
+    TORCH_CHECK(chunks.is_contiguous() && chunks.dim() == 2 && chunks.size(1) == 2, "chunks must be int64 [n_chunks, 2]");
+    const int64_t n_chunks = chunks.size(0);
+    TORCH_CHECK(n_chunks * 128 < (int64_t)INT32_MAX, "too many hub chunks");
+    TORCH_CHECK(part.is_cuda() && part.scalar_type() == at::kFloat && part.is_contiguous() && part.numel() >= n_chunks * p.kp_nbr,
+                "part must be fp32 [>= n_chunks * kp_nbr]");
+    TORCH_CHECK((reinterpret_cast<uintptr_t>(part.data_ptr()) & 15) == 0, "part must be 16 B aligned");
+    p.hub_map = hmap.data_ptr<int>();
+    p.hub_cptr = cptr.data_ptr<int>();
+    p.hub_part = part.data_ptr<float>();
+    p.hub_stride = p.kp_nbr;
+    if (n_chunks > 0) {
+      const int vec = p.tnbr.dtype == 0 ? 4 : 8;
+      const int lanes_row = p.kp_nbr / vec;
+      const int64_t warps = n_chunks * (lanes_row > 32 ? lanes_row / 32 : 1);
+      const unsigned grid = (unsigned)((warps * 32 + 255) / 256);
+      const int64_t* ch = chunks.data_ptr<int64_t>();
+      float* pt = part.data_ptr<float>();
+      if (p.tnbr.dtype == 0)
+        sage_hub_partial_kernel<kCsrU, 0><<<grid, 256, 0, stream>>>(p.tnbr, p.wshift_nbr, p.csr_indices, ch, (int)n_chunks, p.kp_nbr, pt, p.zero_row);
+      else if (p.tnbr.dtype == 1)
+        sage_hub_partial_kernel<kCsrU, 1><<<grid, 256, 0, stream>>>(p.tnbr, p.wshift_nbr, p.csr_indices, ch, (int)n_chunks, p.kp_nbr, pt, p.zero_row);
+      else
+        sage_hub_partial_kernel<kCsrU, 2><<<grid, 256, 0, stream>>>(p.tnbr, p.wshift_nbr, p.csr_indices, ch, (int)n_chunks, p.kp_nbr, pt, p.zero_row);
+      C10_CUDA_KERNEL_LAUNCH_CHECK();
+    }
+  }
+  p.dbg = g_dbg_ptr;
+  plan_tiles(p, sm_count());
+  launch_persist(p, smem, sm_count(), stream, true);
 }
 
 // single-segment convenience wrapper (autograd op in ops/sage.py)

@@ -143,6 +143,7 @@ class FastSageTrainer:
             e.record()
         # root traversal driving step_query (installed by from_query / a subclass), its next-epoch prefetch thread
         self._q_iter = self._q_thread = self._q_next = None
+        self._inf = None                # infer_all: (CSR plan, local vids, hidden-layer tables), built on first call
 
     # ------------------------------------------------------------------ GSL front end
     @classmethod
@@ -552,6 +553,59 @@ class FastSageTrainer:
         out = self.model.forward_store(self.nodes, hops, self.fanouts)
         self.model.train()
         return out
+
+    @torch.no_grad()
+    def infer_all(self) -> torch.Tensor:
+        """Layer-wise full-neighbourhood forward of the trained model: fp32 ``[n_local, out_dim]`` for every local node
+        of the node table, row r = the node with vid ``r * world + rank`` (logits of a supervised trainer, embeddings of
+        a link trainer).  Layer l aggregates the FULL adjacency row of every node in ``self.csr`` (the neighbourhood
+        training samples from) over the outputs of layer l - 1: one fused launch per layer, plus one hub pre-pass
+        launch per layer when the CSR has rows above ``ops.sage.CSR_HUB_DEGREE``.  It uses the resident weight images
+        and the training forward's layer semantics (hidden layers ReLU -> bf16, top layer fp32), is deterministic and is
+        the expectation that the sampled ``predict`` estimates.  Training state is not touched.  Collective when
+        world > 1 (the hidden-layer tables are symmetric, allocated on the first call).  Export::
+
+            from graphlearn_b200.utils.checkpoint import save_embeddings
+            ids = tr.nodes.idmap.to_id(tr.nodes.idmap.local_vids())
+            save_embeddings(path, ids, tr.infer_all())
+        """
+        from ..parallel.runtime import make_table_desc
+        rt, n = self.rt, self.nodes.n_local
+        if self._inf is None:
+            plan = sage_ops.CsrPlan(self.csr.indptr.local, self.csr.indices.local, n)
+            tabs = []
+            for c in self.convs[:-1]:
+                stride = (c.out_dim + 7) // 8 * 8                  # 16-byte bf16 rows
+                st = rt.symm_empty((n, stride), torch.bfloat16)
+                tabs.append((st, make_table_desc(rt.world, c.out_dim, stride, torch.bfloat16, st.nrows, st.ptrs)))
+            rt.barrier()
+            self._inf = (plan, self.nodes.idmap.local_vids(), tabs)
+        plan, vids, tabs = self._inf
+        rt.barrier()                                                # peers are done reading the previous call's tables
+        desc = self.nodes.feat_desc
+        for l in range(1, self.L + 1):
+            c = self.convs[l - 1]
+            last = l == self.L
+            ns, N = self.n_split[l - 1], self.n_img[l - 1]
+            n_out = c.out_dim if ns == 1 else N             # N-split layers: image i writes columns [i N, i N + N)
+            if last:
+                res = torch.empty(n, c.out_dim if ns == 1 else ns * N, dtype=torch.float32, device=rt.device)
+                out = res[:, :n_out]
+            else:
+                out = tabs[l - 1][0].local[:, :n_out]
+            plan.layer(desc, desc, vids, out, c.agg_type, self.img[l - 1], c.bias, N, n_out, not last, not last, ns)
+            if not last:
+                desc = tabs[l - 1][1]
+                rt.barrier()                                        # layer l + 1 reads peer rows of layer l
+        return res[:, :self.convs[-1].out_dim]
+
+    @torch.no_grad()
+    def evaluate(self, vids: torch.Tensor) -> float:
+        """Accuracy of the argmax of the ``infer_all()`` rows of the local nodes `vids` (device int64) against the node
+        table's labels (supervised trainers)."""
+        rows = torch.div(vids, self.rt.world, rounding_mode="floor")
+        pred = self.infer_all()[rows].argmax(1)
+        return float((pred == self.nodes.labels.local[rows]).float().mean())
 
     def state_dict(self):
         return {"model": self.flat_p.clone(), "opt": self.opt.state_dict(), "rng": self.rng.state_dict(),

@@ -66,6 +66,62 @@ def smem_fits(k_total: int, n_pad: int) -> bool:
     return smem_bytes(k_total, n_pad) <= _SMEM_LIMIT
 
 
+# CSR mode of the fused layer (layer-wise full-neighbourhood inference).  A row with more than CSR_HUB_DEGREE neighbours
+# is a hub: a pre-pass sums its adjacency in chunks of CSR_HUB_CHUNK edges (one warp each) and the layer reads the
+# chunks' fp32 partial rows instead.  Why 256: a 64-row tile of products-like rows (mean degree ~50) is ~3 500 row reads,
+# ~180 per gather warp, and the double-buffered A tile lets one warp fall about one tile's share behind before its CTA
+# waits; a 256-neighbour row is ~1.5 shares, while a 3 000-neighbour row would hold the CTA for ~15 tiles.
+CSR_HUB_DEGREE = 256
+CSR_HUB_CHUNK = 256
+
+
+class CsrPlan:
+    """Static inputs of the CSR mode for one adjacency: row m of a layer aggregates the vids
+    ``indices[indptr[m] .. indptr[m + 1])``.  Built once per CSR (hub list, pre-pass chunks, tile-costing degree);
+    ``layer`` then runs one layer over all ``n_rows`` rows with no allocation after the first call per width."""
+
+    def __init__(self, indptr: torch.Tensor, indices: torch.Tensor, n_rows: int, hub_degree: int = CSR_HUB_DEGREE):
+        dev = indices.device
+        n_csr = int(indptr.numel()) - 1
+        if n_csr < n_rows:                  # rows without an adjacency row have degree 0
+            indptr = torch.cat([indptr, indptr[-1:].expand(n_rows - n_csr)])
+        self.indptr = indptr[:n_rows + 1].contiguous()
+        self.indices = indices.contiguous()
+        deg = self.indptr[1:] - self.indptr[:-1]
+        hub = deg > hub_degree
+        rows = hub.nonzero().flatten()
+        self.n_hub = int(rows.numel())
+        light = deg[~hub]
+        self.plan_deg = max(1, int(round(float(light.double().mean())))) if light.numel() else 1
+        self.n_chunks = 0
+        self.hubs = []
+        if self.n_hub:
+            nch = (deg[rows] + CSR_HUB_CHUNK - 1) // CSR_HUB_CHUNK
+            cptr = torch.zeros(self.n_hub + 1, dtype=torch.int64, device=dev)
+            cptr[1:] = torch.cumsum(nch, 0)
+            self.n_chunks = int(cptr[-1])
+            owner = torch.repeat_interleave(torch.arange(self.n_hub, device=dev), nch)
+            start = self.indptr[rows][owner] + (torch.arange(self.n_chunks, device=dev) - cptr[owner]) * CSR_HUB_CHUNK
+            end = torch.minimum(start + CSR_HUB_CHUNK, self.indptr[rows + 1][owner])
+            hub_map = torch.full((n_rows,), -1, dtype=torch.int32, device=dev)
+            hub_map[rows] = torch.arange(self.n_hub, dtype=torch.int32, device=dev)
+            self.hubs = [hub_map, cptr.to(torch.int32), torch.stack([start, end], 1).contiguous()]
+        self._part = {}                     # padded width -> fp32 partial rows of the hub chunks
+
+    def layer(self, tself_desc, tnbr_desc, self_vids: torch.Tensor, out: torch.Tensor, mode: str, w_img: torch.Tensor,
+              bias: Optional[torch.Tensor], N: int, n_out: int, relu: bool, out_bf16: bool, n_imgs: int = 1):
+        """One fused layer over every row: out[m] = act([x_self(self_vids[m]) || agg over the CSR row m] . W^T + b).
+        One launch, preceded by the hub pre-pass launch when the CSR has hubs."""
+        hubs = []
+        if self.hubs:
+            kp = pad_k(int(tnbr_desc[1]))
+            if kp not in self._part:
+                self._part[kp] = torch.empty(self.n_chunks * kp, dtype=torch.float32, device=self.indices.device)
+            hubs = self.hubs + [self._part[kp]]
+        native().sage_fused_csr(tself_desc, tnbr_desc, self_vids, self.indptr, self.indices, hubs, out, MODE[mode], w_img,
+                                bias, N, n_out, relu, out_bf16, n_imgs, self.plan_deg)
+
+
 def logical_weight(weight_p: torch.Tensor, d_self: int, d_nbr: int, mode: str) -> torch.Tensor:
     """[n_out, d_self + d_nbr] (or [n_out, d] for gcn) view of a padded weight."""
     kp_self, _ = padded_dims(d_self, d_nbr, mode)
