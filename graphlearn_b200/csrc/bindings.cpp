@@ -44,6 +44,7 @@ int sm_count();
 void sage_set_debug_trace(const c10::optional<at::Tensor>&);
 // sage_bwd.cu
 at::Tensor pack_weight_t(const at::Tensor&, int64_t, int64_t);
+void sage_bwd_da(const at::Tensor&, const at::Tensor&, int64_t, const at::Tensor&);
 void sage_bwd_dw(const c10::optional<at::Tensor>&, const c10::optional<at::Tensor>&, const std::vector<int64_t>&,
                  const std::vector<int64_t>&, const std::vector<c10::optional<at::Tensor>>&,
                  const std::vector<c10::optional<at::Tensor>>&, const std::vector<int64_t>&, const std::vector<double>&, int64_t,
@@ -182,6 +183,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("sage_set_debug_trace", &glb::sage_set_debug_trace);
   m.def("pack_weight_t", &glb::pack_weight_t);
   m.def("sage_bwd_dw", &glb::sage_bwd_dw);
+  m.def("sage_bwd_da", &glb::sage_bwd_da);
   m.def("pack_weight_f32", &glb::pack_weight_f32);
   m.def("tc_linear_forward", &glb::tc_linear_forward);
   m.def("softmax_ce", &glb::softmax_ce);

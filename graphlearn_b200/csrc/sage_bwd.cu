@@ -387,4 +387,90 @@ void sage_bwd_dw(const c10::optional<at::Tensor>& dz, const c10::optional<at::Te
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
 
+// ------------------------------------------------------------------------------------------------
+// dA = dZ . W of a layer with at most 64 output columns (the top layer of the flagship: 47 classes / a 64-wide
+// embedding), on warp-level mma.sync m16n8k16 (bf16 in, fp32 accumulate).  The general path - the persistent forward
+// kernel over a K-major image of W^T - pays its whole-chip prologue (W^T image TMA of every CTA, barrier setup, a
+// gather role for rows that are plain dZ rows) for 25 M FMA; here a CTA stages one 64-column block of the forward image
+// W [N rows x 64 K columns], SW128, 8 KB at N = 64, and its 4 warps each multiply 16 dZ rows with it.  The B fragments come
+// from the image by ldmatrix.trans: each 8x8 matrix is 8 consecutive image rows at one 16-byte chunk, which the swizzle
+// spreads over 8 different bank groups.
+// grid = (K_total / 64, ceil(rows / 64)), 128 threads.
+constexpr int kDaThreads = 128;
+
+__global__ void __launch_bounds__(kDaThreads) sage_bwd_da_kernel(const __nv_bfloat16* __restrict__ dz, int ld_dz, int rows,
+                                                                 const uint8_t* __restrict__ w_img, int N,
+                                                                 __nv_bfloat16* __restrict__ da, int ld_da) {
+  __shared__ __align__(128) uint8_t sW[64 * 128];
+  const int kb = blockIdx.x;
+  const uint4* src = reinterpret_cast<const uint4*>(w_img + (size_t)kb * N * 128);
+  for (int i = threadIdx.x; i < N * 8; i += kDaThreads) reinterpret_cast<uint4*>(sW)[i] = __ldg(src + i);
+  __syncthreads();
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int g = lane >> 2, t = lane & 3;
+  const int r0 = blockIdx.y * 64 + warp * 16 + g, r1 = r0 + 8;
+  if (blockIdx.y * 64 + warp * 16 >= rows) return;
+  // A fragments of the warp's 16 rows x N columns of dZ: bf16 pairs 8 ks + t (+ 4) = columns 16 ks + 2 t, + 1 (+ 8)
+  const uint32_t* z0 = reinterpret_cast<const uint32_t*>(dz + (size_t)r0 * ld_dz);
+  const uint32_t* z1 = reinterpret_cast<const uint32_t*>(dz + (size_t)r1 * ld_dz);
+  uint32_t a[4][4];
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks) {
+    const bool in = 16 * ks < N;
+    a[ks][0] = in && r0 < rows ? __ldg(z0 + 8 * ks + t) : 0u;
+    a[ks][1] = in && r1 < rows ? __ldg(z1 + 8 * ks + t) : 0u;
+    a[ks][2] = in && r0 < rows ? __ldg(z0 + 8 * ks + t + 4) : 0u;
+    a[ks][3] = in && r1 < rows ? __ldg(z1 + 8 * ks + t + 4) : 0u;
+  }
+  const uint32_t w_base = gmma::smem_u32(sW);
+#pragma unroll
+  for (int c0 = 0; c0 < 64; c0 += 16) {
+    float acc[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks) {
+      if (16 * ks < N) {
+        uint32_t b[4];
+        const uint32_t row = (uint32_t)(16 * ks + (lane & 15)), col = (uint32_t)(c0 + (lane >> 4) * 8);
+        asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
+                     : "=r"(b[0]), "=r"(b[1]), "=r"(b[2]), "=r"(b[3]) : "r"(w_base + gmma::sw128_offset(row, col)));
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+                       "{%0, %1, %2, %3};"
+                       : "+f"(acc[h][0]), "+f"(acc[h][1]), "+f"(acc[h][2]), "+f"(acc[h][3])
+                       : "r"(a[ks][0]), "r"(a[ks][1]), "r"(a[ks][2]), "r"(a[ks][3]), "r"(b[2 * h]), "r"(b[2 * h + 1]));
+      }
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int c = kb * 64 + c0 + 8 * h + 2 * t;
+      if (r0 < rows) *reinterpret_cast<uint32_t*>(da + (size_t)r0 * ld_da + c) = pack_bf16x2(acc[h][0], acc[h][1]);
+      if (r1 < rows) *reinterpret_cast<uint32_t*>(da + (size_t)r1 * ld_da + c) = pack_bf16x2(acc[h][2], acc[h][3]);
+    }
+  }
+}
+
+// dA [rows, K_total] = dZ [rows, >= N] . W with W given as its forward (K-major SW128) image of N <= 64 output columns
+// ([K_total / 64][N][64], zero rows beyond the real outputs); dZ columns [n_out, N) must be zero or finite.
+void sage_bwd_da(const at::Tensor& dz, const at::Tensor& w_img, int64_t N, const at::Tensor& da) {
+  TORCH_CHECK(N % 16 == 0 && N >= 16 && N <= 64, "sage_bwd_da needs a weight image of 16..64 output columns (multiple of 16)");
+  TORCH_CHECK(dz.is_cuda() && dz.scalar_type() == at::kBFloat16 && dz.dim() == 2 && dz.stride(1) == 1 && dz.size(1) >= N &&
+              dz.stride(0) % 2 == 0 && (reinterpret_cast<uintptr_t>(dz.data_ptr()) & 3) == 0,
+              "dz must be a 4-byte aligned bf16 [rows, >= N] view with an even row stride");
+  const int64_t rows = dz.size(0), k_total = da.size(1);
+  TORCH_CHECK(da.is_cuda() && da.scalar_type() == at::kBFloat16 && da.dim() == 2 && da.size(0) == rows && da.stride(1) == 1 &&
+              da.stride(0) % 2 == 0 && (reinterpret_cast<uintptr_t>(da.data_ptr()) & 3) == 0 && k_total % 64 == 0 && k_total >= 64,
+              "da must be a 4-byte aligned bf16 [rows, K_total] view, K_total a multiple of 64");
+  TORCH_CHECK(w_img.is_cuda() && w_img.scalar_type() == at::kBFloat16 && w_img.is_contiguous() && w_img.numel() == k_total * N &&
+              (reinterpret_cast<uintptr_t>(w_img.data_ptr()) & 15) == 0, "w_img must be the 16-byte aligned [K_total / 64][N][64] image");
+  TORCH_CHECK(rows < (int64_t)INT32_MAX / 2, "too many rows");
+  if (rows == 0) return;
+  c10::cuda::CUDAGuard guard(dz.device());
+  const dim3 grid((unsigned)(k_total / 64), (unsigned)((rows + 63) / 64));
+  sage_bwd_da_kernel<<<grid, kDaThreads, 0, at::cuda::getCurrentCUDAStream()>>>(
+      bf16_ptr(dz), (int)dz.stride(0), (int)rows, reinterpret_cast<const uint8_t*>(w_img.data_ptr()), (int)N,
+      reinterpret_cast<__nv_bfloat16*>(da.data_ptr()), (int)da.stride(0));
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+}
+
 }  // namespace glb

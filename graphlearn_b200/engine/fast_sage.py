@@ -9,7 +9,8 @@ pre-allocated buffers (static shapes -> CUDA graph friendly):
         (multi-segment); the top layer's launch also computes softmax-CE, dlogits and the bias gradient
   for l = L..1:  dW_l = dZ_l^T A_l   split-K wgmma kernel, fp32 accumulation straight into the flat gradient buffer;
                                      for l < L, dZ_l = relu'(H_l) * (self + nbr/k rows of dA_{l+1}) is computed by its producers
-                 dA_l = dZ_l W_l     the forward kernel with a K-major image of W_l^T                      [l > 1]
+                 dA_l = dZ_l W_l     [l > 1] a top layer of <= 64 columns in one image: a small mma.sync kernel over its
+                                     forward image; otherwise the forward kernel with a K-major image of W_l^T
   K8    ONE kernel: peer-memory all-reduce (world > 1) + Adam + gradient zeroing + bf16 weight images of the next step
 
 9 launches of this repo's kernels (0 library kernels) for the 2-layer flagship instead of ~60 on the autograd path.
@@ -82,6 +83,9 @@ class FastSageTrainer:
             assert sage_ops.fused_supported(c.in_self, c.in_nbr, min(c.out_dim, n_img), c.agg_type, max(self.fanouts))
             self.n_split.append(ns)
             self.n_img.append(n_img)
+        # dA_L = dZ_L W_L of a top layer of <= 64 columns in one image runs on the small sage_bwd_da kernel over the
+        # forward image (no W^T image); wider or split top layers use the forward kernel with a W^T image
+        self._small_top_da = self.L > 1 and self.n_split[-1] == 1 and self.n_img[-1] <= 64
         # per layer l (1-based): segments i = 0..L-l, rows concatenated
         self.seg_off: List[List[int]] = []
         self.H: List[Optional[torch.Tensor]] = []      # layer outputs (bf16; last layer fp32 logits)
@@ -117,9 +121,10 @@ class FastSageTrainer:
             N = self.n_split[l - 1] * self.n_img[l - 1]
             self.img.append(torch.zeros(kt * N, dtype=torch.bfloat16, device=dev))
             kpad = self.dZp[l - 1].size(1)
-            self.img_t.append(torch.zeros((kt + 255) // 256, kpad * 256, dtype=torch.bfloat16, device=dev) if l > 1 else None)
+            wt = l > 1 and not (l == self.L and self._small_top_da)
+            self.img_t.append(torch.zeros((kt + 255) // 256, kpad * 256, dtype=torch.bfloat16, device=dev) if wt else None)
             mats.append([model._glb_param_offsets[id(c.weight_p)], n_out, kt, self.n_img[l - 1], self.img[-1].data_ptr(),
-                         self.img_t[-1].data_ptr() if l > 1 else 0, kpad, 256])
+                         self.img_t[-1].data_ptr() if wt else 0, kpad, 256])
         self._mats = torch.tensor(mats, dtype=torch.int64)
         self.loss_out = torch.zeros(1, dtype=torch.float32, device=dev)
         self.repack()
@@ -390,7 +395,10 @@ class FastSageTrainer:
                 C.sage_bwd_dw(None, self.H[l - 1], r0, r1, selfs, nbrs, ks, scales, kp_self_n,
                               self.dZ[l - 1] if l >= 2 else None, a, c.weight_p.grad,
                               c.bias.grad if c.bias is not None else None, c.out_dim)
-            if l >= 2:
+            if l == L and self._small_top_da:
+                # dA_L [rows, K_total] = dZ_L [rows, n_out] . W_L on the small mma.sync kernel over the forward image
+                C.sage_bwd_da(self.dZp[l - 1], self.img[l - 1], self.n_img[l - 1], self.dA[l - 1])
+            elif l >= 2:
                 # dA_l [rows, K_total] = dZ_l [rows, n_out] . W_l, one launch per 256-column block
                 dzp = self.dZp[l - 1]
                 d = local_table_desc(dzp)
@@ -437,7 +445,7 @@ class FastSageTrainer:
                 self.img[l - 1].copy_(torch.cat([self.C.pack_weight_f32(wpad[i * N:(i + 1) * N].contiguous(), N, False)[0] for i in range(ns)]))
             else:
                 self.img[l - 1].copy_(self.C.pack_weight_f32(w, N, False)[0])
-            if l > 1:
+            if self.img_t[l - 1] is not None:
                 self.img_t[l - 1].copy_(self.C.pack_weight_t(c.weight_p.detach().contiguous(), self.dZp[l - 1].size(1), 256))
 
     # ------------------------------------------------------------------ graph / public step (same API as SageTrainer)
