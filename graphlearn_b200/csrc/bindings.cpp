@@ -36,15 +36,14 @@ void sage_fused_multi(const at::Tensor&, const at::Tensor&, const std::vector<c1
                       const std::vector<int64_t>&, const std::vector<int64_t>&, const std::vector<at::Tensor>&,
                       const std::vector<c10::optional<at::Tensor>>&, int64_t, const at::Tensor&,
                       const c10::optional<at::Tensor>&, int64_t, int64_t, bool, bool,
-                      const std::vector<c10::optional<at::Tensor>>&, int64_t, int64_t, int64_t);
+                      const std::vector<c10::optional<at::Tensor>>&, int64_t, int64_t);
 void sage_fused_csr(const at::Tensor&, const at::Tensor&, const at::Tensor&, const at::Tensor&, const at::Tensor&,
                     const std::vector<at::Tensor>&, const at::Tensor&, int64_t, const at::Tensor&,
                     const c10::optional<at::Tensor>&, int64_t, int64_t, bool, bool, int64_t, int64_t);
 int sm_count();
 void sage_set_debug_trace(const c10::optional<at::Tensor>&);
 // sage_bwd.cu
-at::Tensor pack_weight_t(const at::Tensor&, int64_t, int64_t);
-void sage_bwd_da(const at::Tensor&, const at::Tensor&, int64_t, const at::Tensor&);
+void sage_bwd_da(const at::Tensor&, const at::Tensor&, int64_t, int64_t, const at::Tensor&);
 void sage_bwd_dw(const c10::optional<at::Tensor>&, const c10::optional<at::Tensor>&, const std::vector<int64_t>&,
                  const std::vector<int64_t>&, const std::vector<c10::optional<at::Tensor>>&,
                  const std::vector<c10::optional<at::Tensor>>&, const std::vector<int64_t>&, const std::vector<double>&, int64_t,
@@ -181,7 +180,6 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("sage_fused_csr", &glb::sage_fused_csr);
   m.def("sm_count", &glb::sm_count);
   m.def("sage_set_debug_trace", &glb::sage_set_debug_trace);
-  m.def("pack_weight_t", &glb::pack_weight_t);
   m.def("sage_bwd_dw", &glb::sage_bwd_dw);
   m.def("sage_bwd_da", &glb::sage_bwd_da);
   m.def("pack_weight_f32", &glb::pack_weight_f32);

@@ -208,7 +208,7 @@ adam_flat_kernel(float* __restrict__ w, const float* __restrict__ g, float* __re
 // Adam fused with everything the next step needs from the parameters (engine/fast_sage.py):
 //   * the gradient (and the scratch accumulators behind it) is zeroed in the same pass - no memset per step
 //   * every weight matrix is re-emitted as the bf16 SWIZZLE_128B K-major image the fused forward kernel feeds
-//     to wgmma (and, for layers >= 2, the image of W^T used by dA = dZ . W) - no pack kernels per step
+//     to wgmma and dA = dZ . W reads - no pack kernels per step
 //   * the loss accumulated by the fused CE epilogue is moved to `loss_out` before it is cleared
 // One thread owns 8 consecutive parameters (parameter starts are 8-aligned in the flat buffer).
 // ---------------------------------------------------------------------------
@@ -219,8 +219,6 @@ struct PackMat {
   int N;                  // rows of ONE forward image per k-block (padded n_out, or n_out / n_imgs for N-split layers);
                           // image i holds the weight rows [i * N, i * N + N)
   uint8_t* img;           // forward image: (k_total/64) k-blocks of [N x 64] bf16, SW128
-  uint8_t* img_t;         // W^T images (or null): [n_imgs][kpad_t/64 k-blocks][nrows_t x 64]
-  int kpad_t, nrows_t;
 };
 struct AdamPackParams {
   float* w; float* g; float* m; float* v;
@@ -375,31 +373,18 @@ __global__ void __launch_bounds__(128) adam_pack_kernel(const __grid_constant__ 
       const size_t off = ((size_t)fi * (pm.k_total >> 6) + kb) * pm.N * 128 + (size_t)(nl >> 3) * 1024 + (size_t)(nl & 7) * 128 +
                          (size_t)((ch ^ (nl & 7)) * 16);
       *reinterpret_cast<uint4*>(pm.img + off) = val;
-      if (pm.img_t) {
-        // W^T image: row = column of W (kcol + i), k index = n
-        const int nkb_t = pm.kpad_t >> 6;
-        const int kbt = n >> 6, cht = (n & 63) >> 3;
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const int col = kcol + i;
-          const int h = col / pm.nrows_t, r = col - h * pm.nrows_t;
-          const size_t o = ((size_t)h * nkb_t + kbt) * pm.nrows_t * 128 + (size_t)(r >> 3) * 1024 + (size_t)(r & 7) * 128 +
-                           (size_t)((cht ^ (r & 7)) * 16) + (size_t)(n & 7) * 2;
-          *reinterpret_cast<__nv_bfloat16*>(pm.img_t + o) = __float2bfloat16(w[i]);
-        }
-      }
     }
   }
 }
 
-// mats: CPU int64 [n_mats, 8] = (off, n_out, k_total, N, img_ptr, img_t_ptr, kpad_t, nrows_t)
+// mats: CPU int64 [n_mats, 5] = (off, n_out, k_total, N, img_ptr)
 void adam_pack(const at::Tensor& w, const at::Tensor& g_store, const at::Tensor& m, const at::Tensor& v, const at::Tensor& step,
                double lr, double beta1, double beta2, double eps, double weight_decay, const c10::optional<at::Tensor>& loss_out,
                const at::Tensor& mats, const c10::optional<at::Tensor>& ar_desc, const c10::optional<at::Tensor>& ar_epochs,
                const c10::optional<at::Tensor>& ar_error, double ar_scale, bool stage_bf16) {
   TORCH_CHECK(w.is_cuda() && w.scalar_type() == at::kFloat && w.is_contiguous() && w.numel() % 8 == 0, "flat params must be padded to 8");
   TORCH_CHECK(g_store.is_cuda() && g_store.scalar_type() == at::kFloat && g_store.numel() >= w.numel() && m.numel() == w.numel() && v.numel() == w.numel());
-  TORCH_CHECK(mats.device().is_cpu() && mats.scalar_type() == at::kLong && mats.dim() == 2 && mats.size(1) == 8 && mats.size(0) <= kMaxPackMats);
+  TORCH_CHECK(mats.device().is_cpu() && mats.scalar_type() == at::kLong && mats.dim() == 2 && mats.size(1) == 5 && mats.size(0) <= kMaxPackMats);
   c10::cuda::CUDAGuard guard(w.device());
   AdamPackParams p;
   std::memset(&p, 0, sizeof(p));
@@ -413,9 +398,8 @@ void adam_pack(const at::Tensor& w, const at::Tensor& g_store, const at::Tensor&
   const int64_t* d = mats.data_ptr<int64_t>();
   for (int i = 0; i < p.n_mats; ++i) {
     PackMat& pm = p.mats[i];
-    pm.off = d[8 * i]; pm.n_out = (int)d[8 * i + 1]; pm.k_total = (int)d[8 * i + 2]; pm.N = (int)d[8 * i + 3];
-    pm.img = reinterpret_cast<uint8_t*>(d[8 * i + 4]); pm.img_t = reinterpret_cast<uint8_t*>(d[8 * i + 5]);
-    pm.kpad_t = (int)d[8 * i + 6]; pm.nrows_t = (int)d[8 * i + 7];
+    pm.off = d[5 * i]; pm.n_out = (int)d[5 * i + 1]; pm.k_total = (int)d[5 * i + 2]; pm.N = (int)d[5 * i + 3];
+    pm.img = reinterpret_cast<uint8_t*>(d[5 * i + 4]);
     TORCH_CHECK(pm.off % 8 == 0 && pm.k_total % 64 == 0, "weight matrices must start 8-aligned with K padded to 64");
   }
   p.world = 1;

@@ -261,47 +261,6 @@ __global__ void __launch_bounds__(kDwThreads, 1) sage_bwd_dw_kernel(const __grid
   }
 }
 
-// fp32 master weight [n_out, k_total] -> bf16 K-major SW128 images of W^T for the dA = dZ . W GEMM:
-// image h (one per 256-column block of k_total) = (K_pad/64) k-blocks of [rows = 256 (columns 256h.. of W), 64 k (= n_out index)]
-__global__ void pack_wt_sw128_kernel(const float* __restrict__ w, int n_out, int k_total, int kpad, int nrows_img,
-                                     uint8_t* __restrict__ img) {
-  const int idx = blockIdx.x * blockDim.x + threadIdx.x;     // one 16-byte chunk (8 k values) of one image row
-  const int nkb = kpad >> 6;
-  const int n_imgs = (k_total + nrows_img - 1) / nrows_img;
-  const int total = n_imgs * nkb * nrows_img * 8;
-  if (idx >= total) return;
-  const int c = idx & 7;
-  const int n = (idx >> 3) % nrows_img;
-  const int kb = ((idx >> 3) / nrows_img) % nkb;
-  const int h = (idx >> 3) / nrows_img / nkb;
-  const int col = h * nrows_img + n;                          // column of W = row of W^T
-  float f[8];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const int kk = kb * 64 + c * 8 + i;                       // row of W
-    f[i] = (col < k_total && kk < n_out) ? w[(size_t)kk * k_total + col] : 0.f;
-  }
-  uint4 val;
-  val.x = pack_bf16x2(f[0], f[1]); val.y = pack_bf16x2(f[2], f[3]); val.z = pack_bf16x2(f[4], f[5]); val.w = pack_bf16x2(f[6], f[7]);
-  const size_t off = ((size_t)h * nkb + kb) * nrows_img * 128 + (size_t)(n >> 3) * 1024 + (size_t)(n & 7) * 128 + (size_t)((c ^ (n & 7)) * 16);
-  *reinterpret_cast<uint4*>(img + off) = val;
-}
-
-// returns the concatenated images [n_imgs, kpad * nrows_img] (bf16)
-at::Tensor pack_weight_t(const at::Tensor& w, int64_t kpad, int64_t nrows_img) {
-  TORCH_CHECK(w.is_cuda() && w.scalar_type() == at::kFloat && w.dim() == 2 && w.is_contiguous());
-  TORCH_CHECK(kpad % 64 == 0 && kpad >= w.size(0) && nrows_img % 8 == 0);
-  c10::cuda::CUDAGuard guard(w.device());
-  const int64_t n_out = w.size(0), k_total = w.size(1);
-  const int64_t n_imgs = (k_total + nrows_img - 1) / nrows_img;
-  auto img = at::empty({n_imgs, kpad * nrows_img}, w.options().dtype(at::kBFloat16));
-  const int total = (int)(n_imgs * (kpad / 64) * nrows_img * 8);
-  pack_wt_sw128_kernel<<<(total + 255) / 256, 256, 0, at::cuda::getCurrentCUDAStream()>>>(
-      w.data_ptr<float>(), (int)n_out, (int)k_total, (int)kpad, (int)nrows_img, reinterpret_cast<uint8_t*>(img.data_ptr()));
-  C10_CUDA_KERNEL_LAUNCH_CHECK();
-  return img;
-}
-
 static const __nv_bfloat16* bf16_ptr(const at::Tensor& t) { return reinterpret_cast<const __nv_bfloat16*>(t.data_ptr()); }
 
 // dW (+)= dZ^T A with dZ either dense (`dz`) or computed from (h, segments of dA_next).
@@ -388,87 +347,132 @@ void sage_bwd_dw(const c10::optional<at::Tensor>& dz, const c10::optional<at::Te
 }
 
 // ------------------------------------------------------------------------------------------------
-// dA = dZ . W of a layer with at most 64 output columns (the top layer of the flagship: 47 classes / a 64-wide
-// embedding), on warp-level mma.sync m16n8k16 (bf16 in, fp32 accumulate).  The general path - the persistent forward
-// kernel over a K-major image of W^T - pays its whole-chip prologue (W^T image TMA of every CTA, barrier setup, a
-// gather role for rows that are plain dZ rows) for 25 M FMA; here a CTA stages one 64-column block of the forward image
-// W [N rows x 64 K columns], SW128, 8 KB at N = 64, and its 4 warps each multiply 16 dZ rows with it.  The B fragments come
-// from the image by ldmatrix.trans: each 8x8 matrix is 8 consecutive image rows at one 16-byte chunk, which the swizzle
-// spreads over 8 different bank groups.
-// grid = (K_total / 64, ceil(rows / 64)), 128 threads.
+// dA = dZ . W of every layer l >= 2, straight from the layer's forward weight images (no W^T copy), on warp-level
+// mma.sync m16n8k16 (bf16 in, fp32 accumulate).  The reduction runs over the R = n_imgs * N rows of the images: image i
+// holds the weight rows [i N, i N + N), zero beyond n_out.  CTA (kb, y) stages the 64-column block kb of every image,
+// [R rows x 64 K columns] SW128 = R * 128 bytes, and its 4 warps each multiply 16 dZ rows with it: A fragments of 4
+// reduction steps in flight, the accumulators of all 64 output columns in registers.  The B fragments come from the block by
+// ldmatrix.trans: each 8x8 matrix is 8 consecutive block rows at one 16-byte chunk, which the swizzle spreads over 8
+// different bank groups (N is a multiple of 8, so the images' swizzle atoms line up in the concatenated block).
+// grid = (K_total / 64, min(ceil(rows / 64), kDaCtasPerSm * SMs / (K_total / 64))) x 128 threads: when there are more row
+// blocks than that, a CTA keeps its W block and walks row blocks y, y + gridDim.y, ... (a wide layer's block is up to
+// 64 KB, and re-staging it for every 64 rows would cost more L2 traffic than the dZ rows themselves).
 constexpr int kDaThreads = 128;
+constexpr int kDaMaxR = 512;
+constexpr int kDaCtasPerSm = 4;
 
 __global__ void __launch_bounds__(kDaThreads) sage_bwd_da_kernel(const __nv_bfloat16* __restrict__ dz, int ld_dz, int rows,
-                                                                 const uint8_t* __restrict__ w_img, int N,
+                                                                 const uint8_t* __restrict__ w_img, int N, int n_imgs,
                                                                  __nv_bfloat16* __restrict__ da, int ld_da) {
-  __shared__ __align__(128) uint8_t sW[64 * 128];
-  const int kb = blockIdx.x;
-  const uint4* src = reinterpret_cast<const uint4*>(w_img + (size_t)kb * N * 128);
-  for (int i = threadIdx.x; i < N * 8; i += kDaThreads) reinterpret_cast<uint4*>(sW)[i] = __ldg(src + i);
-  __syncthreads();
+  extern __shared__ __align__(128) uint8_t sW[];
+  const int kb = blockIdx.x, nkb = gridDim.x;
+  const int R = n_imgs * N;
+  const uint32_t w_base = gmma::smem_u32(sW);
+  // the W block arrives by cp.async, overlapped with the first dZ loads
+  for (int i = 0; i < n_imgs; ++i) {
+    const uint8_t* src = w_img + ((size_t)i * nkb + kb) * N * 128;
+    for (int j = threadIdx.x; j < N * 8; j += kDaThreads)
+      asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(w_base + (uint32_t)(i * N * 128 + j * 16)), "l"(src + j * 16));
+  }
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int g = lane >> 2, t = lane & 3;
-  const int r0 = blockIdx.y * 64 + warp * 16 + g, r1 = r0 + 8;
-  if (blockIdx.y * 64 + warp * 16 >= rows) return;
-  // A fragments of the warp's 16 rows x N columns of dZ: bf16 pairs 8 ks + t (+ 4) = columns 16 ks + 2 t, + 1 (+ 8)
-  const uint32_t* z0 = reinterpret_cast<const uint32_t*>(dz + (size_t)r0 * ld_dz);
-  const uint32_t* z1 = reinterpret_cast<const uint32_t*>(dz + (size_t)r1 * ld_dz);
-  uint32_t a[4][4];
+  bool staged = false;
+  for (int rb = blockIdx.y; rb * 64 + warp * 16 < rows || !staged; rb += gridDim.y) {
+    const bool live = rb * 64 + warp * 16 < rows;                // warp-uniform
+    const int r0 = rb * 64 + warp * 16 + g, r1 = r0 + 8;
+    const bool ok0 = live && r0 < rows, ok1 = live && r1 < rows;
+    // A fragment of reduction step ks: bf16 pairs 8 ks + t (+ 4) = dZ columns 16 ks + 2 t, + 1 (+ 8); loaded 4 steps at a
+    // time, the next 4 in flight while the current 4 are multiplied
+    const uint32_t* z0 = reinterpret_cast<const uint32_t*>(dz + (size_t)(ok0 ? r0 : 0) * ld_dz);
+    const uint32_t* z1 = reinterpret_cast<const uint32_t*>(dz + (size_t)(ok1 ? r1 : 0) * ld_dz);
+    auto load = [&](int ks0, uint32_t (&a)[4][4]) {
 #pragma unroll
-  for (int ks = 0; ks < 4; ++ks) {
-    const bool in = 16 * ks < N;
-    a[ks][0] = in && r0 < rows ? __ldg(z0 + 8 * ks + t) : 0u;
-    a[ks][1] = in && r1 < rows ? __ldg(z1 + 8 * ks + t) : 0u;
-    a[ks][2] = in && r0 < rows ? __ldg(z0 + 8 * ks + t + 4) : 0u;
-    a[ks][3] = in && r1 < rows ? __ldg(z1 + 8 * ks + t + 4) : 0u;
-  }
-  const uint32_t w_base = gmma::smem_u32(sW);
-#pragma unroll
-  for (int c0 = 0; c0 < 64; c0 += 16) {
-    float acc[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
-#pragma unroll
-    for (int ks = 0; ks < 4; ++ks) {
-      if (16 * ks < N) {
-        uint32_t b[4];
-        const uint32_t row = (uint32_t)(16 * ks + (lane & 15)), col = (uint32_t)(c0 + (lane >> 4) * 8);
-        asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
-                     : "=r"(b[0]), "=r"(b[1]), "=r"(b[2]), "=r"(b[3]) : "r"(w_base + gmma::sw128_offset(row, col)));
-#pragma unroll
-        for (int h = 0; h < 2; ++h)
-          asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
-                       "{%0, %1, %2, %3};"
-                       : "+f"(acc[h][0]), "+f"(acc[h][1]), "+f"(acc[h][2]), "+f"(acc[h][3])
-                       : "r"(a[ks][0]), "r"(a[ks][1]), "r"(a[ks][2]), "r"(a[ks][3]), "r"(b[2 * h]), "r"(b[2 * h + 1]));
+      for (int j = 0; j < 4; ++j) {
+        const int ks = ks0 + j;
+        const bool in = 16 * ks < R;
+        a[j][0] = in && ok0 ? __ldg(z0 + 8 * ks + t) : 0u;
+        a[j][1] = in && ok1 ? __ldg(z1 + 8 * ks + t) : 0u;
+        a[j][2] = in && ok0 ? __ldg(z0 + 8 * ks + t + 4) : 0u;
+        a[j][3] = in && ok1 ? __ldg(z1 + 8 * ks + t + 4) : 0u;
       }
+    };
+    uint32_t a[4][4], an[4][4];
+    load(0, a);
+    if (!staged) {
+      asm volatile("cp.async.wait_all;" ::: "memory");
+      __syncthreads();
+      staged = true;
+      if (!live) break;
+    }
+    float acc[8][4];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) acc[j][0] = acc[j][1] = acc[j][2] = acc[j][3] = 0.f;
+    for (int ks0 = 0; ks0 < R / 16; ks0 += 4) {
+      if (ks0 + 4 < R / 16) load(ks0 + 4, an);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        if (16 * (ks0 + j) < R) {
+#pragma unroll
+          for (int c0 = 0; c0 < 4; ++c0) {
+            uint32_t b[4];
+            const uint32_t row = (uint32_t)(16 * (ks0 + j) + (lane & 15)), col = (uint32_t)(16 * c0 + (lane >> 4) * 8);
+            asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
+                         : "=r"(b[0]), "=r"(b[1]), "=r"(b[2]), "=r"(b[3]) : "r"(w_base + gmma::sw128_offset(row, col)));
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              float* c = acc[2 * c0 + h];
+              asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+                           "{%0, %1, %2, %3};"
+                           : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+                           : "r"(a[j][0]), "r"(a[j][1]), "r"(a[j][2]), "r"(a[j][3]), "r"(b[2 * h]), "r"(b[2 * h + 1]));
+            }
+          }
+        }
+      }
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+#pragma unroll
+        for (int q = 0; q < 4; ++q) a[j][q] = an[j][q];
     }
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int c = kb * 64 + c0 + 8 * h + 2 * t;
-      if (r0 < rows) *reinterpret_cast<uint32_t*>(da + (size_t)r0 * ld_da + c) = pack_bf16x2(acc[h][0], acc[h][1]);
-      if (r1 < rows) *reinterpret_cast<uint32_t*>(da + (size_t)r1 * ld_da + c) = pack_bf16x2(acc[h][2], acc[h][3]);
+    for (int j = 0; j < 8; ++j) {
+      const int c = kb * 64 + 8 * j + 2 * t;
+      if (ok0) *reinterpret_cast<uint32_t*>(da + (size_t)r0 * ld_da + c) = pack_bf16x2(acc[j][0], acc[j][1]);
+      if (ok1) *reinterpret_cast<uint32_t*>(da + (size_t)r1 * ld_da + c) = pack_bf16x2(acc[j][2], acc[j][3]);
     }
   }
 }
 
-// dA [rows, K_total] = dZ [rows, >= N] . W with W given as its forward (K-major SW128) image of N <= 64 output columns
-// ([K_total / 64][N][64], zero rows beyond the real outputs); dZ columns [n_out, N) must be zero or finite.
-void sage_bwd_da(const at::Tensor& dz, const at::Tensor& w_img, int64_t N, const at::Tensor& da) {
-  TORCH_CHECK(N % 16 == 0 && N >= 16 && N <= 64, "sage_bwd_da needs a weight image of 16..64 output columns (multiple of 16)");
-  TORCH_CHECK(dz.is_cuda() && dz.scalar_type() == at::kBFloat16 && dz.dim() == 2 && dz.stride(1) == 1 && dz.size(1) >= N &&
+// dA [rows, K_total] = dZ [rows, >= R] . W with W given as its n_imgs forward (K-major SW128) images of N output columns
+// each ([n_imgs][K_total / 64][N][64], zero rows beyond the real outputs), R = n_imgs * N; dZ columns [n_out, R) must be
+// zero or finite.
+void sage_bwd_da(const at::Tensor& dz, const at::Tensor& w_img, int64_t N, int64_t n_imgs, const at::Tensor& da) {
+  const int64_t R = n_imgs * N;
+  TORCH_CHECK(N % 8 == 0 && N >= 8 && n_imgs >= 1 && R % 32 == 0 && R <= kDaMaxR,
+              "sage_bwd_da needs n_imgs images of N output columns (N a multiple of 8), n_imgs * N a multiple of 32 in [32, ",
+              kDaMaxR, "]");
+  TORCH_CHECK(dz.is_cuda() && dz.scalar_type() == at::kBFloat16 && dz.dim() == 2 && dz.stride(1) == 1 && dz.size(1) >= R &&
               dz.stride(0) % 2 == 0 && (reinterpret_cast<uintptr_t>(dz.data_ptr()) & 3) == 0,
-              "dz must be a 4-byte aligned bf16 [rows, >= N] view with an even row stride");
+              "dz must be a 4-byte aligned bf16 [rows, >= n_imgs * N] view with an even row stride");
   const int64_t rows = dz.size(0), k_total = da.size(1);
   TORCH_CHECK(da.is_cuda() && da.scalar_type() == at::kBFloat16 && da.dim() == 2 && da.size(0) == rows && da.stride(1) == 1 &&
               da.stride(0) % 2 == 0 && (reinterpret_cast<uintptr_t>(da.data_ptr()) & 3) == 0 && k_total % 64 == 0 && k_total >= 64,
               "da must be a 4-byte aligned bf16 [rows, K_total] view, K_total a multiple of 64");
-  TORCH_CHECK(w_img.is_cuda() && w_img.scalar_type() == at::kBFloat16 && w_img.is_contiguous() && w_img.numel() == k_total * N &&
-              (reinterpret_cast<uintptr_t>(w_img.data_ptr()) & 15) == 0, "w_img must be the 16-byte aligned [K_total / 64][N][64] image");
+  TORCH_CHECK(w_img.is_cuda() && w_img.scalar_type() == at::kBFloat16 && w_img.is_contiguous() && w_img.numel() == k_total * R &&
+              (reinterpret_cast<uintptr_t>(w_img.data_ptr()) & 15) == 0,
+              "w_img must be the 16-byte aligned [n_imgs][K_total / 64][N][64] images");
   TORCH_CHECK(rows < (int64_t)INT32_MAX / 2, "too many rows");
   if (rows == 0) return;
   c10::cuda::CUDAGuard guard(dz.device());
-  const dim3 grid((unsigned)(k_total / 64), (unsigned)((rows + 63) / 64));
-  sage_bwd_da_kernel<<<grid, kDaThreads, 0, at::cuda::getCurrentCUDAStream()>>>(
-      bf16_ptr(dz), (int)dz.stride(0), (int)rows, reinterpret_cast<const uint8_t*>(w_img.data_ptr()), (int)N,
+  static bool attr_done = false;
+  if (!attr_done) {
+    C10_CUDA_CHECK(cudaFuncSetAttribute(sage_bwd_da_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kDaMaxR * 128));
+    attr_done = true;
+  }
+  const int64_t nkb = k_total / 64, row_blocks = (rows + 63) / 64;
+  const dim3 grid((unsigned)nkb, (unsigned)std::min<int64_t>(row_blocks, std::max<int64_t>(1, kDaCtasPerSm * sm_count() / nkb)));
+  sage_bwd_da_kernel<<<grid, kDaThreads, (size_t)R * 128, at::cuda::getCurrentCUDAStream()>>>(
+      bf16_ptr(dz), (int)dz.stride(0), (int)rows, reinterpret_cast<const uint8_t*>(w_img.data_ptr()), (int)N, (int)n_imgs,
       reinterpret_cast<__nv_bfloat16*>(da.data_ptr()), (int)da.stride(0));
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }

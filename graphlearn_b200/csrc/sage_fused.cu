@@ -95,7 +95,7 @@ struct SageParams {
   int ce_dl_stride;
   float* ce_dbias;            // [n_out] accumulated, or null
   float ce_inv_b;
-  // several weight images in one launch (dA = dZ . W with K_total > 256): CTA b uses image b % n_imgs, walks the tiles
+  // several weight images in one launch (an N-split layer): CTA b uses image b % n_imgs, walks the tiles
   // b / n_imgs + j * (gridDim.x / n_imgs) and writes output columns [img * N, img * N + n_out)
   int n_imgs;
   long long* dbg;             // optional [grid][64] clock64 trace (tools/persist_timeline.py), lane 0 of one warp per role
@@ -850,8 +850,8 @@ static const char* zero_row_for(const at::TensorOptions& opts, int dev) {
 
 // Balanced tiling: every tile should cost about the same number of row fetches ((k + 1) per destination
 // row, + 2 for the epilogue / A stores) and the tile count should just fill `waves` tiles per SM.
-static void plan_tiles(SageParams& p, int usable_sms) {
-  const int sms = std::max(1, usable_sms / p.n_imgs);
+static void plan_tiles(SageParams& p) {
+  const int sms = std::max(1, sm_count() / p.n_imgs);
   int64_t n128 = 0;
   double total_cost = 0.0;
   for (int s = 0; s < p.nseg; ++s) {
@@ -886,9 +886,9 @@ static void launch_one(const SageParams& p, unsigned grid, size_t smem, cudaStre
 // row loads in flight per lane of the CSR mode (one instantiation per table dtype)
 constexpr int kCsrU = 5;
 
-static void launch_persist(SageParams& p, size_t smem, int usable_sms, cudaStream_t stream, bool csr = false) {
+static void launch_persist(SageParams& p, size_t smem, cudaStream_t stream, bool csr = false) {
   if (p.total_tiles == 0) return;
-  const unsigned grid = (unsigned)(p.n_imgs * std::min<int>(std::max(1, usable_sms / p.n_imgs), p.total_tiles));
+  const unsigned grid = (unsigned)(p.n_imgs * std::min<int>(std::max(1, sm_count() / p.n_imgs), p.total_tiles));
   int kmax = 1;
   for (int s = 0; s < p.nseg; ++s) kmax = std::max(kmax, p.seg[s].k);
   const int dt = p.tnbr.dtype;
@@ -959,7 +959,6 @@ static void set_seg_out(SageParams& p, SageSeg& sg, const at::Tensor& out, int64
 // a_saves[i] ([M_i, K_total] bf16, the [self || agg] rows for the backward pass).
 // ce = optional fused softmax cross-entropy on the output rows of segment 0:
 //   [labels_table(int64), seeds(int64)|undefined, loss(fp32 >=1), dlogits(bf16 [M, stride]), dbias(fp32)|undefined]
-// max_ctas caps the grid (0 = one CTA per SM), leaving SMs to a kernel that should run beside this launch.
 void sage_fused_multi(const at::Tensor& tself_desc, const at::Tensor& tnbr_desc,
                       const std::vector<c10::optional<at::Tensor>>& self_vids,
                       const std::vector<c10::optional<at::Tensor>>& nbr_vids,
@@ -968,7 +967,7 @@ void sage_fused_multi(const at::Tensor& tself_desc, const at::Tensor& tnbr_desc,
                       const std::vector<at::Tensor>& outs, const std::vector<c10::optional<at::Tensor>>& a_saves,
                       int64_t mode, const at::Tensor& w_img, const c10::optional<at::Tensor>& bias, int64_t N,
                       int64_t n_out, bool relu, bool out_bf16,
-                      const std::vector<c10::optional<at::Tensor>>& ce, int64_t ce_world, int64_t n_imgs, int64_t max_ctas) {
+                      const std::vector<c10::optional<at::Tensor>>& ce, int64_t ce_world, int64_t n_imgs) {
   TORCH_CHECK(w_img.is_cuda() && w_img.scalar_type() == at::kBFloat16, "w_img must be CUDA bf16");
   c10::cuda::CUDAGuard guard(w_img.device());
   const int nseg = (int)Ms.size();
@@ -1041,9 +1040,8 @@ void sage_fused_multi(const at::Tensor& tself_desc, const at::Tensor& tnbr_desc,
     p.ce_inv_b = 1.f / (float)Ms[0];
   }
   p.dbg = g_dbg_ptr;
-  const int usable_sms = max_ctas > 0 ? std::min<int>(sm_count(), (int)max_ctas) : sm_count();
-  plan_tiles(p, usable_sms);
-  launch_persist(p, smem, usable_sms, at::cuda::getCurrentCUDAStream());
+  plan_tiles(p);
+  launch_persist(p, smem, at::cuda::getCurrentCUDAStream());
 }
 
 // Layer-wise full-neighbourhood inference: ONE layer over every row of a CSR (row m of `out` aggregates the neighbour
@@ -1112,8 +1110,8 @@ void sage_fused_csr(const at::Tensor& tself_desc, const at::Tensor& tnbr_desc, c
     }
   }
   p.dbg = g_dbg_ptr;
-  plan_tiles(p, sm_count());
-  launch_persist(p, smem, sm_count(), stream, true);
+  plan_tiles(p);
+  launch_persist(p, smem, stream, true);
 }
 
 // single-segment convenience wrapper (autograd op in ops/sage.py)
@@ -1136,7 +1134,7 @@ std::vector<at::Tensor> sage_fused_forward(const at::Tensor& tself_desc,
   if (M == 0) return {out, a_save};
   sage_fused_multi(tself_desc, tnbr_desc, {self_vids}, {nbr_vids}, {0}, {0}, {M}, {k}, {out},
                    {save_a ? c10::optional<at::Tensor>(a_save) : c10::nullopt}, mode, w_img, bias, N, n_out, relu, out_bf16,
-                   {}, 1, 1, 0);
+                   {}, 1, 1);
   return {out, a_save};
 }
 
@@ -1155,7 +1153,7 @@ at::Tensor tc_linear_forward(const at::Tensor& a, const at::Tensor& w_img, const
   d[0] = 1; d[1] = K; d[2] = a.stride(0); d[3] = 1; d[4] = M; d[4 + kMaxWorld] = reinterpret_cast<int64_t>(a.data_ptr());
   at::Tensor desc = at::from_blob(d.data(), {(int64_t)d.size()}, at::kLong).clone();
   sage_fused_multi(desc, desc, {c10::nullopt}, {c10::nullopt}, {0}, {0}, {M}, {0}, {out}, {c10::nullopt}, kConcatMean, w_img, bias,
-                   N, n_out, relu, out_bf16, {}, 1, 1, 0);
+                   N, n_out, relu, out_bf16, {}, 1, 1);
   return out;
 }
 

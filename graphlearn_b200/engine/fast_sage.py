@@ -9,8 +9,7 @@ pre-allocated buffers (static shapes -> CUDA graph friendly):
         (multi-segment); the top layer's launch also computes softmax-CE, dlogits and the bias gradient
   for l = L..1:  dW_l = dZ_l^T A_l   split-K wgmma kernel, fp32 accumulation straight into the flat gradient buffer;
                                      for l < L, dZ_l = relu'(H_l) * (self + nbr/k rows of dA_{l+1}) is computed by its producers
-                 dA_l = dZ_l W_l     [l > 1] a top layer of <= 64 columns in one image: a small mma.sync kernel over its
-                                     forward image; otherwise the forward kernel with a K-major image of W_l^T
+                 dA_l = dZ_l W_l     [l > 1] mma.sync kernel over the layer's forward weight images
   K8    ONE kernel: peer-memory all-reduce (world > 1) + Adam + gradient zeroing + bf16 weight images of the next step
 
 9 launches of this repo's kernels (0 library kernels) for the 2-layer flagship instead of ~60 on the autograd path.
@@ -83,9 +82,6 @@ class FastSageTrainer:
             assert sage_ops.fused_supported(c.in_self, c.in_nbr, min(c.out_dim, n_img), c.agg_type, max(self.fanouts))
             self.n_split.append(ns)
             self.n_img.append(n_img)
-        # dA_L = dZ_L W_L of a top layer of <= 64 columns in one image runs on the small sage_bwd_da kernel over the
-        # forward image (no W^T image); wider or split top layers use the forward kernel with a W^T image
-        self._small_top_da = self.L > 1 and self.n_split[-1] == 1 and self.n_img[-1] <= 64
         # per layer l (1-based): segments i = 0..L-l, rows concatenated
         self.seg_off: List[List[int]] = []
         self.H: List[Optional[torch.Tensor]] = []      # layer outputs (bf16; last layer fp32 logits)
@@ -113,18 +109,13 @@ class FastSageTrainer:
             self.dA.append(torch.zeros(rows, kt, dtype=torch.bfloat16, device=dev) if l > 1 else None)
         # persistent bf16 weight images (written by the fused Adam kernel at the end of every step)
         self.img: List[torch.Tensor] = []
-        self.img_t: List[Optional[torch.Tensor]] = []
         mats = []
         for l in range(1, self.L + 1):
             c = convs[l - 1]
             n_out, kt = c.weight_p.shape
             N = self.n_split[l - 1] * self.n_img[l - 1]
             self.img.append(torch.zeros(kt * N, dtype=torch.bfloat16, device=dev))
-            kpad = self.dZp[l - 1].size(1)
-            wt = l > 1 and not (l == self.L and self._small_top_da)
-            self.img_t.append(torch.zeros((kt + 255) // 256, kpad * 256, dtype=torch.bfloat16, device=dev) if wt else None)
-            mats.append([model._glb_param_offsets[id(c.weight_p)], n_out, kt, self.n_img[l - 1], self.img[-1].data_ptr(),
-                         self.img_t[-1].data_ptr() if wt else 0, kpad, 256])
+            mats.append([model._glb_param_offsets[id(c.weight_p)], n_out, kt, self.n_img[l - 1], self.img[-1].data_ptr()])
         self._mats = torch.tensor(mats, dtype=torch.int64)
         self.loss_out = torch.zeros(1, dtype=torch.float32, device=dev)
         self.repack()
@@ -295,7 +286,7 @@ class FastSageTrainer:
             sampling: on main (plain schedule) or, under graph capture, the NEXT batch on its own branch, followed by
                       the rng + optimiser step counters
             main    : one persistent launch per layer (all hop pairs of the layer; the top layer also computes the loss)
-            side A  : dW_L GEMM   ||   main : dA_L (forward kernel with the W^T image) -> dW_{L-1} (dZ computed on the fly) ...
+            side A  : dW_L GEMM   ||   main : dA_L (sage_bwd_da) -> dW_{L-1} (dZ computed on the fly) -> dA_{L-1} ...
         everything joins before ONE fused kernel: gradient all-reduce + Adam + grad zeroing + next step's weight images."""
         C, L = self.C, self.L
         main = torch.cuda.current_stream()
@@ -357,7 +348,7 @@ class FastSageTrainer:
                 self_ids = nbr_ids = [None] * nseg
                 self_base, nbr_base = self.seg_off[l - 2][:nseg], self.seg_off[l - 2][1:nseg + 1]
             C.sage_fused_multi(d, d, self_ids, nbr_ids, self_base, nbr_base, Ms, ks, outs, asv, mode, img, c.bias, N,
-                               n_out, not last, not last, ce, self.rt.world, ns, 0)
+                               n_out, not last, not last, ce, self.rt.world, ns)
             if last and not fuse_ce:
                 # wide / split top layer: the loss runs as its own kernel on the (padded) logits
                 self._top_loss(seeds)
@@ -370,7 +361,7 @@ class FastSageTrainer:
         #   top layer   : dW_L = dZ_L^T A_L with the dense dZ_L written by the fused loss epilogue
         #   layer l < L : dW_l = dZ_l^T A_l where dZ_l = relu'(H_l) * (self + 1/k neighbour rows of dA_{l+1}) is
         #                 computed inside the GEMM's producer warps (never stored for l = 1); bias grads fall out
-        #   dA_l = dZ_l . W_l  (l >= 2) on the persistent forward kernel with a K-major image of W_l^T
+        #   dA_l = dZ_l . W_l  (l >= 2) on sage_bwd_da (mma.sync) over the layer's forward weight images
         for l in range(L, 0, -1):
             c = self.convs[l - 1]
             a = self.A[l - 1]
@@ -395,23 +386,9 @@ class FastSageTrainer:
                 C.sage_bwd_dw(None, self.H[l - 1], r0, r1, selfs, nbrs, ks, scales, kp_self_n,
                               self.dZ[l - 1] if l >= 2 else None, a, c.weight_p.grad,
                               c.bias.grad if c.bias is not None else None, c.out_dim)
-            if l == L and self._small_top_da:
-                # dA_L [rows, K_total] = dZ_L [rows, n_out] . W_L on the small mma.sync kernel over the forward image
-                C.sage_bwd_da(self.dZp[l - 1], self.img[l - 1], self.n_img[l - 1], self.dA[l - 1])
-            elif l >= 2:
-                # dA_l [rows, K_total] = dZ_l [rows, n_out] . W_l, one launch per 256-column block
-                dzp = self.dZp[l - 1]
-                d = local_table_desc(dzp)
-                wt = self.img_t[l - 1]
-                da = self.dA[l - 1]
-                rows = da.size(0)
-                # one launch: CTA b multiplies by image b % n_imgs and writes the columns [256 img, 256 img + 256)
-                n_imgs = wt.size(0)
-                cols = min(256, da.size(1))
-                # dW_L (<= 32 whole-SM CTAs for a 1024-row top layer) runs beside the dA_L launch: leave it its SMs
-                max_ctas = max(C.sm_count() - 32, C.sm_count() // 2) if l == L else 0
-                C.sage_fused_multi(d, d, [None], [None], [0], [0], [rows], [0], [da[:, :cols]], [None], 0, wt, None, 256, cols,
-                                   False, True, [], 1, n_imgs, max_ctas)
+            if l >= 2:
+                # dA_l [rows, K_total] = dZ_l [rows, n_split * n_img] . W_l
+                C.sage_bwd_da(self.dZp[l - 1], self.img[l - 1], self.n_img[l - 1], self.n_split[l - 1], self.dA[l - 1])
         # ---- join, gradient all-reduce + fused optimiser (Adam + zero grads + next step's weight images)
         main.wait_stream(sA)
         if pipe is not None:
@@ -445,8 +422,6 @@ class FastSageTrainer:
                 self.img[l - 1].copy_(torch.cat([self.C.pack_weight_f32(wpad[i * N:(i + 1) * N].contiguous(), N, False)[0] for i in range(ns)]))
             else:
                 self.img[l - 1].copy_(self.C.pack_weight_f32(w, N, False)[0])
-            if self.img_t[l - 1] is not None:
-                self.img_t[l - 1].copy_(self.C.pack_weight_t(c.weight_p.detach().contiguous(), self.dZp[l - 1].size(1), 256))
 
     # ------------------------------------------------------------------ graph / public step (same API as SageTrainer)
     def capture(self, warmup: int = 3):

@@ -219,11 +219,11 @@ def test_infer_all_equals_predict_when_sampling_draws_every_neighbour(rt, link):
 # ------------------------------------------------------------------------------------- 5. training is unaffected
 def _training_state(tr):
     st = [tr.flat_p, tr.g_store, tr.opt.m, tr.opt.v, tr.opt.step_t, tr.rng.state, tr.loss_out] + tr.img + \
-         [t for t in tr.img_t if t is not None] + [t for hop in tr._hops for t in hop]
+         [t for hop in tr._hops for t in hop]
     return [t.clone() for t in st] + [tr._steps]
 
 
-def test_infer_all_leaves_training_untouched(rt):
+def test_infer_all_leaves_training_state_untouched(rt):
     from graphlearn_b200.engine import FastSageTrainer
     from graphlearn_b200.models.graphsage import EgoGraphSAGE
     from graphlearn_b200.store.synthetic import make_sharded_graph

@@ -26,19 +26,19 @@ def card():
         return "nvidia-smi unavailable (%s)" % e
 
 
-def label(name, seen):
-    """stable short name; the launches of one kernel in a step are told apart by their order (L1, L2 + CE and, for a top
-    layer wider than 64 columns, dA for the persistent kernel; dW2 then dW1 for the weight-gradient kernel)"""
+def label(name, seen, L):
+    """stable short name; the launches of one kernel in a step are told apart by their order: the persistent kernel runs
+    the forward L1..L<L>, the backward runs dA<L>..dA2 and dW<L>..dW1"""
     base = name.split("(")[0].replace("void ", "").replace("glb::", "")
     base = base.split("<")[0]
     i = seen.get(base, 0)
     seen[base] = i + 1
     if base == "sage_persist_kernel":
-        return ["L1", "L2+CE", "dA"][min(i, 2)] if i < 3 else "sage_persist#%d" % i
+        return "L%d" % (i + 1)
     if base == "sage_bwd_da_kernel":
-        return "dA"
+        return "dA%d" % (L - i)
     if base == "sage_bwd_dw_kernel":
-        return ["dW2", "dW1"][i] if i < 2 else "dW#%d" % i
+        return "dW%d" % (L - i)
     if base == "sample_neighbors_kernel":
         return "sample_hop%d" % (i + 1)
     return base
@@ -87,14 +87,18 @@ def main():
     seen = {}
     rows = []
     for e in rep:
-        rows.append((label(e.name, seen), e.time_range.start - t0, e.time_range.end - t0, getattr(e, "device_resource_id", None)))
+        rows.append((label(e.name, seen, tr.L), e.time_range.start - t0, e.time_range.end - t0, getattr(e, "device_resource_id", None)))
     print("replay: %d kernels, first start -> adam_pack end %.1f us; adam_pack end to end of the next %.1f us" %
           (len(rep), rows[-1][2], evs[ends[-2]].time_range.end - evs[ends[-3]].time_range.end))
     print("%-18s %9s %9s %8s  %s" % ("kernel", "start us", "end us", "dur us", "stream"))
     for name, s, e, st in rows:
         print("%-18s %9.1f %9.1f %8.1f  %s" % (name, s, e, e - s, st))
-    # main chain: previous replay's adam_pack -> L1 -> L2 + CE -> dA2 -> dW1 -> adam_pack (dW2 runs beside dA2)
-    chain = [n for n in ("L1", "L2+CE", "dA", "dW1", "adam_pack_kernel") if any(r[0] == n for r in rows)]
+    # main chain: previous replay's adam_pack -> L1 .. L<L> (-> softmax_ce) -> dA<L> -> dW<L-1> -> dA<L-1> .. dA2 -> dW1
+    # -> adam_pack (dW<L> runs beside dA<L>)
+    L = tr.L
+    order = ["L%d" % l for l in range(1, L + 1)] + ["softmax_ce_kernel"]
+    order += [n for l in range(L, 1, -1) for n in ("dA%d" % l, "dW%d" % (l - 1))] + ["adam_pack_kernel"]
+    chain = [n for n in order if any(r[0] == n for r in rows)]
     by = {r[0]: r for r in rows}
     prev_end = evs[ends[-3]].time_range.end - t0
     busy = gaps = 0.0
