@@ -91,6 +91,9 @@ def main(argv=None):
         ps = g.runtime.all_gather_object(tr.flat_p.detach().cpu())
         assert all(torch.allclose(p, ps[0], atol=1e-6) for p in ps), "replicas diverged"
         print("replicas in sync on %d ranks" % g.runtime.world)
+        # leave the process group before the interpreter exits: a rank that exits with it alive can abort in the
+        # teardown of its gloo threads ("terminate called without an active exception")
+        g.runtime.shutdown()
     return test_acc
 
 

@@ -111,9 +111,9 @@ class FastLinkSageTrainer(FastSageTrainer):
                                roots[2 * B:])
 
     def _top_loss(self, seeds: torch.Tensor):
-        top = self.convs[-1]
-        self.C.link_loss(self.H[-1], self.batch_size, self.neg_num, LOSS_KINDS[self.loss_kind], self.temperature,
-                         self.loss, self.dZ[-1], top.bias.grad if top.bias is not None else None)
+        top = self.layers[-1]
+        self.C.link_loss(top.H, self.batch_size, self.neg_num, LOSS_KINDS[self.loss_kind], self.temperature,
+                         self.loss, top.dZ, top.db)
 
     def _fill_slot(self, slot: int, first: torch.Tensor, dst: Optional[torch.Tensor] = None):
         """pinned staging slot: [0, B) src vids or CSR positions, [B, 2B) dst vids, [2B] what [0, B) holds"""

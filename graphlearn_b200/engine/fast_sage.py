@@ -25,6 +25,7 @@ compiled GSL query), ``predict``, ``state_dict``.
 """
 from __future__ import annotations
 
+from dataclasses import dataclass
 from typing import List, Optional, Sequence
 
 import torch
@@ -35,6 +36,38 @@ from ..ops import sage as sage_ops
 from ..ops import sampling as S
 from ..parallel.runtime import Runtime, local_table_desc, native
 from ..store.shards import CsrShard, NodeTable
+
+
+@dataclass
+class SageLayer:
+    """Layer l (1-based) of a ``FastSageTrainer``, described once at construction: shape facts, buffers and the launch
+    arguments that do not change between steps.  The layer runs the hop pairs (i, i + 1), i = 0..nseg - 1, as the
+    segments of one launch; segment i is the rows ``offs[i]:offs[i + 1]`` of each of its buffers."""
+    conv: torch.nn.Module
+    last: bool
+    mode: int                       # sage_ops.MODE of the aggregation
+    kt: int                         # padded K: columns of weight_p and of the A / dA rows
+    ns: int                         # forward weight images (N-split when W does not fit next to the A tiles)
+    N: int                          # padded output columns per image
+    n_out: int                      # columns one image writes: out_dim, or N when the layer is N-split
+    nseg: int
+    offs: List[int]
+    rows: int
+    fuse_ce: bool                   # the forward launch computes softmax-CE, dZ and the bias gradient in its epilogue
+    Hp: torch.Tensor                # output with the rows padded to the image columns (bf16; top layer fp32 logits)
+    H: torch.Tensor                 # ... its out_dim real columns
+    A: torch.Tensor                 # saved [self || agg] tiles (bf16)
+    dZp: torch.Tensor               # dZ with the row padded to the K padding of the dA GEMM
+    dZ: torch.Tensor
+    dA: Optional[torch.Tensor]      # None for layer 1
+    img: torch.Tensor               # bf16 weight images (rewritten by the fused Adam kernel at the end of every step)
+    dW: torch.Tensor                # the weight's and the bias's views of the flat gradient buffer
+    db: Optional[torch.Tensor]
+    below: Optional[torch.Tensor]   # table descriptor of H of the layer below; None for layer 1 (feature table, hop ids)
+    fwd: tuple                      # sage_fused_multi's (self_base, nbr_base, Ms, ks, outs, a_saves)
+    # sage_bwd_dw's (seg_row0, seg_row1, self_src, nbr_src, seg_k, seg_scale, nbr_col0, dz_out) for l < L, where dZ_l is
+    # computed from dA of the layer above
+    bwd: Optional[tuple] = None
 
 
 class FastSageTrainer:
@@ -66,57 +99,56 @@ class FastSageTrainer:
         self.n = [self.B]
         for k in self.fanouts:
             self.n.append(self.n[-1] * k)
-        convs = list(model.convs)
-        self.convs = convs
-        self.n_split: List[int] = []           # forward images per layer (N-split when W does not fit next to the A tiles)
-        self.n_img: List[int] = []             # padded output columns per image
-        for c in convs:
+        self.convs = list(model.convs)
+        self.layers: List[SageLayer] = []
+        for l, c in enumerate(self.convs, 1):
             assert c.agg_type in ("mean", "sum"), "fast engine supports mean / sum aggregation"
-            kt = c.weight_p.size(1)
-            ns, n_img = 1, sage_ops.pad_n(c.out_dim)
-            while not sage_ops.smem_fits(kt, n_img) and ns < 8:          # fewest images whose W slice fits next to the A tiles
-                ns += 1
-                n_img = (-(-c.out_dim // ns) + 31) // 32 * 32
-            is_top = c is convs[-1]
-            assert sage_ops.smem_fits(kt, n_img) and (ns == 1 or is_top or ns * n_img == c.out_dim), "layer does not fit the fused kernel"
-            assert sage_ops.fused_supported(c.in_self, c.in_nbr, min(c.out_dim, n_img), c.agg_type, max(self.fanouts))
-            self.n_split.append(ns)
-            self.n_img.append(n_img)
-        # per layer l (1-based): segments i = 0..L-l, rows concatenated
-        self.seg_off: List[List[int]] = []
-        self.H: List[Optional[torch.Tensor]] = []      # layer outputs (bf16; last layer fp32 logits)
-        self.Hp: List[torch.Tensor] = []               # ... with the rows padded to the image columns
-        self.A: List[torch.Tensor] = []                # saved [self || agg] tiles (bf16)
-        self.dZ: List[torch.Tensor] = []
-        self.dZp: List[torch.Tensor] = []              # dZ with the row padded to the K padding of the dA GEMM
-        self.dA: List[Optional[torch.Tensor]] = []
-        for l in range(1, self.L + 1):
-            c = convs[l - 1]
-            segs = self.L - l + 1
-            offs = [0]
-            for i in range(segs):
-                offs.append(offs[-1] + self.n[i])
-            rows = offs[-1]
-            self.seg_off.append(offs)
             last = l == self.L
             kt = c.weight_p.size(1)
-            hw = self.n_split[l - 1] * self.n_img[l - 1] if last else c.out_dim      # padded logits rows (all images)
-            self.Hp.append(torch.zeros(rows, hw, dtype=torch.float32 if last else torch.bfloat16, device=dev))
-            self.H.append(self.Hp[-1][:, :c.out_dim])
-            self.A.append(torch.zeros(rows, kt, dtype=torch.bfloat16, device=dev))
-            self.dZp.append(torch.zeros(rows, sage_ops.pad_k(c.out_dim), dtype=torch.bfloat16, device=dev))
-            self.dZ.append(self.dZp[-1][:, :c.out_dim])
-            self.dA.append(torch.zeros(rows, kt, dtype=torch.bfloat16, device=dev) if l > 1 else None)
-        # persistent bf16 weight images (written by the fused Adam kernel at the end of every step)
-        self.img: List[torch.Tensor] = []
-        mats = []
-        for l in range(1, self.L + 1):
-            c = convs[l - 1]
-            n_out, kt = c.weight_p.shape
-            N = self.n_split[l - 1] * self.n_img[l - 1]
-            self.img.append(torch.zeros(kt * N, dtype=torch.bfloat16, device=dev))
-            mats.append([model._glb_param_offsets[id(c.weight_p)], n_out, kt, self.n_img[l - 1], self.img[-1].data_ptr()])
-        self._mats = torch.tensor(mats, dtype=torch.int64)
+            ns, N = sage_ops.split_images(kt, c.out_dim)
+            assert sage_ops.smem_fits(kt, N) and (ns == 1 or last or ns * N == c.out_dim), "layer does not fit the fused kernel"
+            assert sage_ops.fused_supported(c.in_self, c.in_nbr, min(c.out_dim, N), c.agg_type, max(self.fanouts))
+            n_out = c.out_dim if ns == 1 else N
+            nseg = self.L - l + 1
+            offs = [0]
+            for i in range(nseg):
+                offs.append(offs[-1] + self.n[i])
+            rows = offs[-1]
+            Hp = torch.zeros(rows, ns * N if last else c.out_dim, dtype=torch.float32 if last else torch.bfloat16, device=dev)
+            A = torch.zeros(rows, kt, dtype=torch.bfloat16, device=dev)
+            dZp = torch.zeros(rows, sage_ops.pad_k(c.out_dim), dtype=torch.bfloat16, device=dev)
+            dA = torch.zeros(rows, kt, dtype=torch.bfloat16, device=dev) if l > 1 else None
+            below, self_base, nbr_base = None, [0] * nseg, [0] * nseg
+            if l > 1:
+                # the segments' self / neighbour rows are the contiguous row ranges of segments i / i + 1 of the layer
+                # below, which in turn takes dZ of its segment s from the self rows of segment s and the neighbour
+                # rows of segment s - 1 of this layer's dA
+                lo = self.layers[-1]
+                below, self_base, nbr_base = local_table_desc(lo.H), lo.offs[:nseg], lo.offs[1:nseg + 1]
+                da_seg = [dA[offs[i]:offs[i + 1]] for i in range(nseg)]
+                k_nbr = self.fanouts[:nseg]
+                scale = [1.0 / k if c.agg_type == "mean" else 1.0 for k in k_nbr]
+                lo.bwd = (lo.offs[:-1], lo.offs[1:], da_seg + [None], [None] + da_seg, [1] + k_nbr, [1.0] + scale,
+                          sage_ops.padded_dims(c.in_self, c.in_nbr, c.agg_type)[0], lo.dZ if lo.dA is not None else None)
+            outs = [Hp[offs[i]:offs[i + 1], :n_out] for i in range(nseg)]
+            a_saves = [A[offs[i]:offs[i + 1]] for i in range(nseg)]
+            self.layers.append(SageLayer(
+                conv=c, last=last, mode=sage_ops.MODE[c.agg_type], kt=kt, ns=ns, N=N, n_out=n_out,
+                nseg=nseg, offs=offs, rows=rows,
+                fuse_ce=last and self._fuse_ce and ns == 1 and N <= 64,
+                Hp=Hp, H=Hp[:, :c.out_dim], A=A, dZp=dZp, dZ=dZp[:, :c.out_dim], dA=dA,
+                img=torch.zeros(kt * ns * N, dtype=torch.bfloat16, device=dev),
+                dW=c.weight_p.grad, db=c.bias.grad if c.bias is not None else None,
+                below=below, fwd=(self_base, nbr_base, self.n[:nseg], self.fanouts[:nseg], outs, a_saves)))
+        # the lists other code reads; they alias the records' tensors
+        self.H = [ly.H for ly in self.layers]
+        self.dA = [ly.dA for ly in self.layers]
+        self.img = [ly.img for ly in self.layers]
+        self.n_split = [ly.ns for ly in self.layers]
+        self.n_img = [ly.N for ly in self.layers]
+        # one row per weight for the fused Adam kernel, which rewrites the images at the end of every step
+        self._mats = torch.tensor([[model._glb_param_offsets[id(ly.conv.weight_p)], ly.conv.out_dim, ly.kt, ly.N,
+                                    ly.img.data_ptr()] for ly in self.layers], dtype=torch.int64)
         self.loss_out = torch.zeros(1, dtype=torch.float32, device=dev)
         self.repack()
         self.graph: Optional[torch.cuda.CUDAGraph] = None
@@ -275,9 +307,8 @@ class FastSageTrainer:
 
     def _top_loss(self, seeds: torch.Tensor):
         """loss, dZ_L and the top bias gradient from the fp32 top-layer output when it was not fused"""
-        top = self.convs[-1]
-        self.C.softmax_ce(self.H[-1], self.nodes.labels.local, seeds, self.rt.world, self.loss, self.dZ[-1],
-                          top.bias.grad if top.bias is not None else None)
+        top = self.layers[-1]
+        self.C.softmax_ce(top.H, self.nodes.labels.local, seeds, self.rt.world, self.loss, top.dZ, top.db)
 
     # ------------------------------------------------------------------ the step
     def _step_body(self, pipe=None):
@@ -288,7 +319,7 @@ class FastSageTrainer:
             main    : one persistent launch per layer (all hop pairs of the layer; the top layer also computes the loss)
             side A  : dW_L GEMM   ||   main : dA_L (sage_bwd_da) -> dW_{L-1} (dZ computed on the fly) -> dA_{L-1} ...
         everything joins before ONE fused kernel: gradient all-reduce + Adam + grad zeroing + next step's weight images."""
-        C, L = self.C, self.L
+        C = self.C
         main = torch.cuda.current_stream()
         sA = self._side
         host_slot = None
@@ -319,37 +350,15 @@ class FastSageTrainer:
                 self.opt.advance(self.rng.state)
         # ---- forward: ONE persistent launch per layer covering all of its hop-pair segments; the top layer's
         # launch also computes the loss, dlogits and the bias gradient in its epilogue (fused CE)
-        top = self.convs[L - 1]
-        for l in range(1, L + 1):
-            c = self.convs[l - 1]
-            last = l == L
-            ns = self.n_split[l - 1]
-            N = self.n_img[l - 1]
-            n_out = c.out_dim if ns == 1 else N
-            img = self.img[l - 1]
-            fuse_ce = last and self._fuse_ce and ns == 1 and N <= 64
-            offs = self.seg_off[l - 1]
-            mode = sage_ops.MODE[c.agg_type]
-            nseg = L - l + 1
-            hb = self.H[l - 1] if ns == 1 else self.Hp[l - 1]
-            outs = [hb[offs[i]:offs[i + 1], :n_out] for i in range(nseg)]
-            asv = [self.A[l - 1][offs[i]:offs[i + 1]] for i in range(nseg)]
-            Ms, ks = [self.n[i] for i in range(nseg)], [self.fanouts[i] for i in range(nseg)]
-            ce = []
-            if fuse_ce:
-                ce = [self.nodes.labels.local, seeds, self.loss, self.dZ[L - 1],
-                      top.bias.grad if top.bias is not None else None]
-            if l == 1:          # self / neighbour rows: ids of hops i / i + 1 in the feature table
-                d = self.nodes.feat_desc
-                self_ids, nbr_ids = hops[:nseg], hops[1:nseg + 1]
-                self_base, nbr_base = [0] * nseg, [0] * nseg
-            else:               # ... the contiguous row ranges of segments i / i + 1 of the layer below
-                d = local_table_desc(self.H[l - 2])
-                self_ids = nbr_ids = [None] * nseg
-                self_base, nbr_base = self.seg_off[l - 2][:nseg], self.seg_off[l - 2][1:nseg + 1]
-            C.sage_fused_multi(d, d, self_ids, nbr_ids, self_base, nbr_base, Ms, ks, outs, asv, mode, img, c.bias, N,
-                               n_out, not last, not last, ce, self.rt.world, ns)
-            if last and not fuse_ce:
+        for ly in self.layers:
+            if ly.below is None:    # self / neighbour rows: ids of hops i / i + 1 in the feature table
+                d, self_ids, nbr_ids = self.nodes.feat_desc, hops[:ly.nseg], hops[1:ly.nseg + 1]
+            else:                   # ... the contiguous row ranges of segments i / i + 1 of the layer below
+                d, self_ids, nbr_ids = ly.below, [None] * ly.nseg, [None] * ly.nseg
+            ce = [self.nodes.labels.local, seeds, self.loss, ly.dZ, ly.db] if ly.fuse_ce else []
+            C.sage_fused_multi(d, d, self_ids, nbr_ids, *ly.fwd, ly.mode, ly.img, ly.conv.bias, ly.N, ly.n_out,
+                               not ly.last, not ly.last, ce, self.rt.world, ly.ns)
+            if ly.last and not ly.fuse_ce:
                 # wide / split top layer: the loss runs as its own kernel on the (padded) logits
                 self._top_loss(seeds)
         if host_slot is not None:
@@ -362,33 +371,16 @@ class FastSageTrainer:
         #   layer l < L : dW_l = dZ_l^T A_l where dZ_l = relu'(H_l) * (self + 1/k neighbour rows of dA_{l+1}) is
         #                 computed inside the GEMM's producer warps (never stored for l = 1); bias grads fall out
         #   dA_l = dZ_l . W_l  (l >= 2) on sage_bwd_da (mma.sync) over the layer's forward weight images
-        for l in range(L, 0, -1):
-            c = self.convs[l - 1]
-            a = self.A[l - 1]
-            if l == L:
+        for ly in reversed(self.layers):
+            if ly.last:
                 sA.wait_stream(main)
                 with torch.cuda.stream(sA):            # dW_L runs beside dA_L
-                    C.sage_bwd_dw(self.dZ[l - 1], None, [], [], [], [], [], [], 0, None, a, c.weight_p.grad, None,
-                                  c.out_dim)
+                    C.sage_bwd_dw(ly.dZ, None, [], [], [], [], [], [], 0, None, ly.A, ly.dW, None, ly.conv.out_dim)
             else:
-                nxt = self.convs[l]
-                da = self.dA[l]
-                offs, po = self.seg_off[l], self.seg_off[l - 1]
-                nseg = L - l + 1
-                kp_self_n, _ = sage_ops.padded_dims(nxt.in_self, nxt.in_nbr, nxt.agg_type)
-                r0 = [po[s] for s in range(nseg)]
-                r1 = [po[s + 1] for s in range(nseg)]
-                selfs = [da[offs[s]:offs[s + 1]] if s <= L - l - 1 else None for s in range(nseg)]
-                nbrs = [da[offs[s - 1]:offs[s]] if s >= 1 else None for s in range(nseg)]
-                ks = [self.fanouts[s - 1] if s >= 1 else 1 for s in range(nseg)]
-                scales = [((1.0 / self.fanouts[s - 1]) if nxt.agg_type == "mean" else 1.0) if s >= 1 else 1.0
-                          for s in range(nseg)]
-                C.sage_bwd_dw(None, self.H[l - 1], r0, r1, selfs, nbrs, ks, scales, kp_self_n,
-                              self.dZ[l - 1] if l >= 2 else None, a, c.weight_p.grad,
-                              c.bias.grad if c.bias is not None else None, c.out_dim)
-            if l >= 2:
+                C.sage_bwd_dw(None, ly.H, *ly.bwd, ly.A, ly.dW, ly.db, ly.conv.out_dim)
+            if ly.dA is not None:
                 # dA_l [rows, K_total] = dZ_l [rows, n_split * n_img] . W_l
-                C.sage_bwd_da(self.dZp[l - 1], self.img[l - 1], self.n_img[l - 1], self.n_split[l - 1], self.dA[l - 1])
+                C.sage_bwd_da(ly.dZp, ly.img, ly.N, ly.ns, ly.dA)
         # ---- join, gradient all-reduce + fused optimiser (Adam + zero grads + next step's weight images)
         main.wait_stream(sA)
         if pipe is not None:
@@ -412,16 +404,8 @@ class FastSageTrainer:
     def repack(self):
         """Rebuild the bf16 weight images from the fp32 master weights (after init / load_state_dict / any
         external modification of the parameters)."""
-        for l in range(1, self.L + 1):
-            c = self.convs[l - 1]
-            ns, N = self.n_split[l - 1], self.n_img[l - 1]
-            w = c.weight_p.detach().contiguous()
-            if ns > 1:
-                wpad = torch.zeros(ns * N, w.size(1), device=w.device)
-                wpad[:w.size(0)] = w
-                self.img[l - 1].copy_(torch.cat([self.C.pack_weight_f32(wpad[i * N:(i + 1) * N].contiguous(), N, False)[0] for i in range(ns)]))
-            else:
-                self.img[l - 1].copy_(self.C.pack_weight_f32(w, N, False)[0])
+        for ly in self.layers:
+            ly.img.copy_(sage_ops.pack_images(ly.conv.weight_p, ly.N, ly.ns))
 
     # ------------------------------------------------------------------ graph / public step (same API as SageTrainer)
     def capture(self, warmup: int = 3):
@@ -566,21 +550,18 @@ class FastSageTrainer:
         plan, vids, tabs = self._inf
         rt.barrier()                                                # peers are done reading the previous call's tables
         desc = self.nodes.feat_desc
-        for l in range(1, self.L + 1):
-            c = self.convs[l - 1]
-            last = l == self.L
-            ns, N = self.n_split[l - 1], self.n_img[l - 1]
-            n_out = c.out_dim if ns == 1 else N             # N-split layers: image i writes columns [i N, i N + N)
-            if last:
-                res = torch.empty(n, c.out_dim if ns == 1 else ns * N, dtype=torch.float32, device=rt.device)
-                out = res[:, :n_out]
+        for l, ly in enumerate(self.layers):
+            c = ly.conv
+            if ly.last:                                             # image i writes columns [i n_out, i n_out + n_out)
+                res = torch.empty(n, ly.ns * ly.n_out, dtype=torch.float32, device=rt.device)
+                out = res[:, :ly.n_out]
             else:
-                out = tabs[l - 1][0].local[:, :n_out]
-            plan.layer(desc, desc, vids, out, c.agg_type, self.img[l - 1], c.bias, N, n_out, not last, not last, ns)
-            if not last:
-                desc = tabs[l - 1][1]
+                out = tabs[l][0].local[:, :ly.n_out]
+            plan.layer(desc, desc, vids, out, c.agg_type, ly.img, c.bias, ly.N, ly.n_out, not ly.last, not ly.last, ly.ns)
+            if not ly.last:
+                desc = tabs[l][1]
                 rt.barrier()                                        # layer l + 1 reads peer rows of layer l
-        return res[:, :self.convs[-1].out_dim]
+        return res[:, :c.out_dim]
 
     @torch.no_grad()
     def evaluate(self, vids: torch.Tensor) -> float:

@@ -66,6 +66,28 @@ def smem_fits(k_total: int, n_pad: int) -> bool:
     return smem_bytes(k_total, n_pad) <= _SMEM_LIMIT
 
 
+def image_width(n_out: int, ns: int) -> int:
+    """Padded output columns N of one forward weight image when the n_out rows of W are N-split over `ns` images."""
+    return pad_n(n_out) if ns == 1 else (-(-n_out // ns) + 31) // 32 * 32
+
+
+def split_images(k_total: int, n_out: int):
+    """(ns, N): the fewest images (at most 8) whose W slice fits in shared memory next to the A tiles.  The caller
+    checks ``smem_fits(k_total, N)``: 8 images may still be too few."""
+    ns = 1
+    while not smem_fits(k_total, image_width(n_out, ns)) and ns < 8:
+        ns += 1
+    return ns, image_width(n_out, ns)
+
+
+def pack_images(weight_p: torch.Tensor, N: int, ns: int) -> torch.Tensor:
+    """The `ns` bf16 SWIZZLE_128B images of a padded fp32 weight ``[n_out, k_total]``, concatenated: image i holds the
+    rows [i N, i N + N) of W, zero rows beyond n_out."""
+    wpad = torch.zeros(ns * N, weight_p.size(1), device=weight_p.device)
+    wpad[:weight_p.size(0)] = weight_p.detach()
+    return torch.cat([native().pack_weight_f32(wpad[i * N:(i + 1) * N], N, False)[0] for i in range(ns)])
+
+
 # CSR mode of the fused layer (layer-wise full-neighbourhood inference).  A row with more than CSR_HUB_DEGREE neighbours
 # is a hub: a pre-pass sums its adjacency in chunks of CSR_HUB_CHUNK edges (one warp each) and the layer reads the
 # chunks' fp32 partial rows instead.  Why 256: a 64-row tile of products-like rows (mean degree ~50) is ~3 500 row reads,

@@ -34,6 +34,9 @@ def test_padded_weight_roundtrip():
     assert wp.shape == (7, 256) and torch.equal(SG.logical_weight(wp, 100, 100, "mean"), w)
     assert float(wp[:, 100:128].abs().sum()) == 0 and float(wp[:, 228:].abs().sum()) == 0
     assert SG.fused_supported(100, 100, 256, "mean") and not SG.fused_supported(600, 600, 256, "mean")
+    # unsplit headline layers (256 hidden, 47 classes over 256 + 256 padded inputs); 172 classes need 3 images of 64 columns
+    assert SG.split_images(256, 256) == (1, 256) and SG.split_images(512, 47) == (1, SG.pad_n(47))
+    assert SG.split_images(512, 172) == (3, 64) and SG.smem_fits(512, 64) and not SG.smem_fits(512, 96)
     # the Python fit check and the kernel's launch check size shared memory with the same formula
     from graphlearn_b200.parallel.runtime import native
     C = native()

@@ -64,10 +64,7 @@ def _layer_ref(xs, agg, w, b, relu):
 def _images(C, w, d, N, ns):
     """weight images of a logical [n_out, 2d] weight, N-split into `ns` images of N columns"""
     from graphlearn_b200.ops import sage as S
-    wp = S.pad_weight(w, d, d, "mean")
-    wpad = torch.zeros(ns * N, wp.size(1), device=w.device)
-    wpad[:wp.size(0)] = wp
-    return torch.cat([C.pack_weight_f32(wpad[i * N:(i + 1) * N].contiguous(), N, False)[0] for i in range(ns)])
+    return S.pack_images(S.pad_weight(w, d, d, "mean"), N, ns)
 
 
 def _run_layer(rt, nodes, indptr, indices, w, b, mode, relu, out_bf16, ns=1, hub_degree=None):
@@ -75,7 +72,7 @@ def _run_layer(rt, nodes, indptr, indices, w, b, mode, relu, out_bf16, ns=1, hub
     from graphlearn_b200.parallel.runtime import native
     C = native()
     n, d, n_real = nodes.n_local, nodes.float_dim, w.size(0)
-    N = S.pad_n(n_real) if ns == 1 else (-(-n_real // ns) + 31) // 32 * 32
+    N = S.image_width(n_real, ns)
     img = _images(C, w, d, N, ns)
     kw = {} if hub_degree is None else {"hub_degree": hub_degree}
     plan = S.CsrPlan(indptr, indices, n, **kw)
