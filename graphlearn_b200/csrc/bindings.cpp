@@ -36,7 +36,8 @@ void sage_fused_multi(const at::Tensor&, const at::Tensor&, const std::vector<c1
                       const std::vector<int64_t>&, const std::vector<int64_t>&, const std::vector<at::Tensor>&,
                       const std::vector<c10::optional<at::Tensor>>&, int64_t, const at::Tensor&,
                       const c10::optional<at::Tensor>&, int64_t, int64_t, bool, bool,
-                      const std::vector<c10::optional<at::Tensor>>&, int64_t, int64_t);
+                      const std::vector<c10::optional<at::Tensor>>&, int64_t, int64_t,
+                      const std::vector<c10::optional<at::Tensor>>&);
 void sage_fused_csr(const at::Tensor&, const at::Tensor&, const at::Tensor&, const at::Tensor&, const at::Tensor&,
                     const std::vector<at::Tensor>&, const at::Tensor&, int64_t, const at::Tensor&,
                     const c10::optional<at::Tensor>&, int64_t, int64_t, bool, bool, int64_t, int64_t);
@@ -47,7 +48,8 @@ void sage_bwd_da(const at::Tensor&, const at::Tensor&, int64_t, int64_t, const a
 void sage_bwd_dw(const c10::optional<at::Tensor>&, const c10::optional<at::Tensor>&, const std::vector<int64_t>&,
                  const std::vector<int64_t>&, const std::vector<c10::optional<at::Tensor>>&,
                  const std::vector<c10::optional<at::Tensor>>&, const std::vector<int64_t>&, const std::vector<double>&, int64_t,
-                 const c10::optional<at::Tensor>&, const at::Tensor&, const at::Tensor&, const c10::optional<at::Tensor>&, int64_t);
+                 const c10::optional<at::Tensor>&, const at::Tensor&, const at::Tensor&, const c10::optional<at::Tensor>&, int64_t,
+                 const std::vector<double>&, const std::vector<c10::optional<at::Tensor>>&);
 // train_ops.cu
 void softmax_ce(const at::Tensor&, const at::Tensor&, const c10::optional<at::Tensor>&, int64_t, const at::Tensor&,
                 const at::Tensor&, const c10::optional<at::Tensor>&);
@@ -176,11 +178,20 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("sparse_adam_rows", &glb::sparse_adam_rows);
   m.def("sage_smem_bytes", &glb::sage_smem_bytes);
   m.def("sage_fused_forward", &glb::sage_fused_forward);
-  m.def("sage_fused_multi", &glb::sage_fused_multi);
+  // (amax: per-segment argmax outputs of a max-aggregating launch, see sage_fused.cu)
+  m.def("sage_fused_multi", &glb::sage_fused_multi, py::arg("tself_desc"), py::arg("tnbr_desc"), py::arg("self_vids"),
+        py::arg("nbr_vids"), py::arg("self_base"), py::arg("nbr_base"), py::arg("Ms"), py::arg("ks"), py::arg("outs"),
+        py::arg("a_saves"), py::arg("mode"), py::arg("w_img"), py::arg("bias"), py::arg("N"), py::arg("n_out"), py::arg("relu"),
+        py::arg("out_bf16"), py::arg("ce"), py::arg("ce_world"), py::arg("n_imgs"),
+        py::arg("amax") = std::vector<c10::optional<at::Tensor>>());
   m.def("sage_fused_csr", &glb::sage_fused_csr);
   m.def("sm_count", &glb::sm_count);
   m.def("sage_set_debug_trace", &glb::sage_set_debug_trace);
-  m.def("sage_bwd_dw", &glb::sage_bwd_dw);
+  // (seg_self_scale / amax_src: the gradient routing of a gcn / max aggregation above, see sage_bwd.cu)
+  m.def("sage_bwd_dw", &glb::sage_bwd_dw, py::arg("dz"), py::arg("h"), py::arg("seg_row0"), py::arg("seg_row1"),
+        py::arg("self_src"), py::arg("nbr_src"), py::arg("seg_k"), py::arg("seg_scale"), py::arg("nbr_col0"), py::arg("dz_out"),
+        py::arg("a"), py::arg("dw"), py::arg("dbias"), py::arg("n_out"), py::arg("seg_self_scale") = std::vector<double>(),
+        py::arg("amax_src") = std::vector<c10::optional<at::Tensor>>());
   m.def("sage_bwd_da", &glb::sage_bwd_da);
   m.def("pack_weight_f32", &glb::pack_weight_f32);
   m.def("tc_linear_forward", &glb::tc_linear_forward);

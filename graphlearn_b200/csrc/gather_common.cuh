@@ -52,6 +52,13 @@ template <> struct Chunk<2> {
     x = e4m3x2_to_float2(v.y);       a[4] = fmaf(x.x, s, a[4]); a[5] = fmaf(x.y, s, a[5]);
     x = e4m3x2_to_float2(v.y >> 16); a[6] = fmaf(x.x, s, a[6]); a[7] = fmaf(x.y, s, a[7]);
   }
+  __device__ __forceinline__ void get(float (&a)[8]) const {     // dequantised
+    float2 x;
+    x = e4m3x2_to_float2(v.x);       a[0] = x.x * s; a[1] = x.y * s;
+    x = e4m3x2_to_float2(v.x >> 16); a[2] = x.x * s; a[3] = x.y * s;
+    x = e4m3x2_to_float2(v.y);       a[4] = x.x * s; a[5] = x.y * s;
+    x = e4m3x2_to_float2(v.y >> 16); a[6] = x.x * s; a[7] = x.y * s;
+  }
 };
 
 // uniform loader: 16-byte chunk `chunk` of a fp32 / bf16 row, or 8-element chunk + block scale of an fp8 row

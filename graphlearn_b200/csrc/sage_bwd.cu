@@ -15,6 +15,10 @@
 //     dZ_l[r, :] = relu'(H_l[r, :]) * ( dA_{l+1}[self row of r, 0:d]  +  scale * dA_{l+1}[parent of r, kp_self : kp_self + d] )
 // so dZ of the big hop segments never exists in HBM for 2-layer models; the bias gradient (column sums of
 // dZ) falls out of the same registers.  Deeper models can ask for dZ to be written (needed by dA = dZ.W).
+// The instantiation ROUTE = true serves the other aggregations of the layer above: a per-segment self scale (gcn:
+// both parts are scaled by 1 / (k + 1)) and, for max, the argmax bytes of the parent row, which pass column c of the
+// neighbour part only to the child j = (r - row0) % k that held the maximum:
+//     dZ_l[r, c] = relu'(H_l[r, c]) * ( sscale * self[c]  +  scale * [amax[parent][c] == j] * nbr[c] )
 //
 // warps 0..15 : producers (loads -> ReLU-grad math -> swizzled st.shared) and, as four warpgroups, the MMA issuers:
 //               warpgroup g owns the [64 x 64] quadrant (rows 64 (g & 1), columns 64 (g >> 1)) of the CTA's dW block
@@ -64,6 +68,10 @@ struct DwParams {
   int rows, n_out, dz_cols, n_cols;
   int m_blocks, n_blocks, rows_per_split;
   uint32_t lbo, sbo, kadv;                  // MN-major descriptor fields (bytes)
+  // ROUTE instantiation only (after the fields above, whose offsets stay put): per segment, the self part's scale and
+  // the argmax rows of the parents (row r -> amax[seg] + ((r - row0) / k) * ld_amax, one byte per column) or null
+  float self_scale[kDwMaxSegs];
+  const uint8_t* amax[kDwMaxSegs]; int ld_amax;
 };
 
 __device__ __forceinline__ uint4 ldg16(const void* p) { return *reinterpret_cast<const uint4*>(p); }
@@ -78,6 +86,7 @@ __device__ __forceinline__ uint32_t mn_off(int r, int c) {
   return (uint32_t)(c >> 3) * 8192u + (uint32_t)(r >> 3) * 1024u + (uint32_t)(r & 7) * 128u + (uint32_t)(((c & 7) ^ (r & 7)) << 4);
 }
 
+template <bool ROUTE>
 __global__ void __launch_bounds__(kDwThreads, 1) sage_bwd_dw_kernel(const __grid_constant__ DwParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (gmma::smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -125,7 +134,9 @@ __global__ void __launch_bounds__(kDwThreads, 1) sage_bwd_dw_kernel(const __grid
     const uint4 zero4 = make_uint4(0u, 0u, 0u, 0u);
     // register-staged operands of one 64-row stage; two sets are alive so that the loads of stage st+1 are in
     // flight while stage st is converted and stored (the kernel is bound by bytes in flight, not by math)
-    struct StageRegs { uint4 bv[2], hv[2], sv[2], nv[2]; float nscale[2]; };
+    // (ROUTE: am = argmax bytes of the chunk's 8 columns, j = this row's index among its parent's children; rows without
+    // an argmax keep am = 0, j = 0, which passes every column)
+    struct StageRegs { uint4 bv[2], hv[2], sv[2], nv[2]; float nscale[2]; uint2 am[2]; uint32_t j[2]; float sscale[2]; };
     auto issue = [&](int st, StageRegs& g) {
       const int rbase = r_begin + st * kDwRows;
 #pragma unroll
@@ -137,6 +148,7 @@ __global__ void __launch_bounds__(kDwThreads, 1) sage_bwd_dw_kernel(const __grid
       for (int i = 0; i < 2; ++i) {
         const int r = rbase + zr + 32 * i;
         g.hv[i] = zero4; g.sv[i] = zero4; g.nv[i] = zero4; g.nscale[i] = 0.f;
+        if constexpr (ROUTE) { g.am[i] = make_uint2(0u, 0u); g.j[i] = 0u; g.sscale[i] = 1.f; }
         if (r < r_end && zcol_ok) {
           if (p.dz) {
             g.sv[i] = ldg16(p.dz + (size_t)r * p.ld_dz + zcol);
@@ -148,6 +160,15 @@ __global__ void __launch_bounds__(kDwThreads, 1) sage_bwd_dw_kernel(const __grid
             const int rl = r - q.row0;
             if (q.self_src) g.sv[i] = ldg16(q.self_src + (size_t)rl * p.ld_da + zcol);
             if (q.nbr_src) { g.nv[i] = ldg16(q.nbr_src + (size_t)(rl / q.k) * p.ld_da + p.nbr_col0 + zcol); g.nscale[i] = q.scale; }
+            if constexpr (ROUTE) {
+              g.sscale[i] = p.self_scale[sg];
+              const uint8_t* am = p.amax[sg];
+              if (am) {
+                const int par = rl / q.k;
+                g.am[i] = *reinterpret_cast<const uint2*>(am + (size_t)par * p.ld_amax + zcol);
+                g.j[i] = (uint32_t)(rl - par * q.k);
+              }
+            }
             if (p.h) g.hv[i] = ldg16(p.h + (size_t)r * p.ld_h + zcol);
           }
         }
@@ -168,7 +189,15 @@ __global__ void __launch_bounds__(kDwThreads, 1) sage_bwd_dw_kernel(const __grid
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
           const float2 a = unpack_bf16x2(ps[j]), b = unpack_bf16x2(pn[j]);
-          float gx = a.x + b.x * g.nscale[i], gy = a.y + b.y * g.nscale[i];
+          float gx, gy;
+          if constexpr (ROUTE) {
+            const uint32_t w = j < 2 ? g.am[i].x : g.am[i].y;            // bytes of columns 2 j, 2 j + 1
+            const uint32_t sh = 16 * (j & 1);
+            const float nx = ((w >> sh) & 0xFFu) == g.j[i] ? b.x : 0.f, ny = ((w >> (sh + 8)) & 0xFFu) == g.j[i] ? b.y : 0.f;
+            gx = a.x * g.sscale[i] + nx * g.nscale[i]; gy = a.y * g.sscale[i] + ny * g.nscale[i];
+          } else {
+            gx = a.x + b.x * g.nscale[i]; gy = a.y + b.y * g.nscale[i];
+          }
           if (p.h) {
             const float2 hh = unpack_bf16x2(ph[j]);
             if (!(hh.x > 0.f)) gx = 0.f;
@@ -263,14 +292,29 @@ __global__ void __launch_bounds__(kDwThreads, 1) sage_bwd_dw_kernel(const __grid
 
 static const __nv_bfloat16* bf16_ptr(const at::Tensor& t) { return reinterpret_cast<const __nv_bfloat16*>(t.data_ptr()); }
 
+template <bool ROUTE>
+static void launch_dw(const DwParams& p, int grid, size_t smem) {
+  static bool attr_done = false;
+  if (!attr_done) {
+    C10_CUDA_CHECK(cudaFuncSetAttribute(sage_bwd_dw_kernel<ROUTE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    attr_done = true;
+  }
+  sage_bwd_dw_kernel<ROUTE><<<grid, kDwThreads, smem, at::cuda::getCurrentCUDAStream()>>>(p);
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+}
+
 // dW (+)= dZ^T A with dZ either dense (`dz`) or computed from (h, segments of dA_next).
 //   segs: rows [row0, row1) of the layer; self_src[i] / nbr_src[i] are views into dA_next (or None)
+//   seg_self_scale: [] (all 1) or the self part's scale per segment (gcn above: 1 / (k + 1))
+//   amax_src: [] or per segment None / the uint8 argmax rows of the parents (max above; aligned with nbr_src[i], >= n_out
+//             columns, row stride a multiple of 8): the neighbour part of column c reaches only the child that held its max
 void sage_bwd_dw(const c10::optional<at::Tensor>& dz, const c10::optional<at::Tensor>& h,
                  const std::vector<int64_t>& seg_row0, const std::vector<int64_t>& seg_row1,
                  const std::vector<c10::optional<at::Tensor>>& self_src, const std::vector<c10::optional<at::Tensor>>& nbr_src,
                  const std::vector<int64_t>& seg_k, const std::vector<double>& seg_scale, int64_t nbr_col0,
                  const c10::optional<at::Tensor>& dz_out, const at::Tensor& a, const at::Tensor& dw,
-                 const c10::optional<at::Tensor>& dbias, int64_t n_out) {
+                 const c10::optional<at::Tensor>& dbias, int64_t n_out, const std::vector<double>& seg_self_scale,
+                 const std::vector<c10::optional<at::Tensor>>& amax_src) {
   TORCH_CHECK(a.is_cuda() && a.scalar_type() == at::kBFloat16 && a.dim() == 2 && a.stride(1) == 1 && a.stride(0) % 8 == 0);
   TORCH_CHECK(dw.is_cuda() && dw.scalar_type() == at::kFloat && dw.dim() == 2 && dw.stride(1) == 1 && dw.size(0) >= n_out &&
               dw.size(1) == a.size(1) && dw.stride(0) % 4 == 0 && (reinterpret_cast<uintptr_t>(dw.data_ptr()) & 15) == 0,
@@ -278,6 +322,7 @@ void sage_bwd_dw(const c10::optional<at::Tensor>& dz, const c10::optional<at::Te
   c10::cuda::CUDAGuard guard(a.device());
   DwParams p;
   std::memset(&p, 0, sizeof(p));
+  bool route = false;
   p.rows = (int)a.size(0); p.n_cols = (int)a.size(1); p.n_out = (int)n_out;
   TORCH_CHECK(p.n_cols % 16 == 0, "K_total must be a multiple of 16");
   p.a = bf16_ptr(a); p.ld_a = (int)a.stride(0);
@@ -314,6 +359,22 @@ void sage_bwd_dw(const c10::optional<at::Tensor>& dz, const c10::optional<at::Te
         else { TORCH_CHECK(src->size(0) * g.k >= g.row1 - g.row0); g.nbr_src = bf16_ptr(*src); }
       }
     }
+    TORCH_CHECK(seg_self_scale.empty() || (int)seg_self_scale.size() == nseg, "seg_self_scale: one entry per segment");
+    TORCH_CHECK(amax_src.empty() || (int)amax_src.size() == nseg, "amax_src: one entry per segment");
+    for (int i = 0; i < nseg; ++i) {
+      p.self_scale[i] = seg_self_scale.empty() ? 1.f : (float)seg_self_scale[i];
+      route = route || p.self_scale[i] != 1.f;
+      if (amax_src.empty() || !(amax_src[i].has_value() && amax_src[i]->defined())) continue;
+      const at::Tensor& m = *amax_src[i];
+      TORCH_CHECK(m.is_cuda() && m.scalar_type() == at::kByte && m.dim() == 2 && m.stride(1) == 1 && m.size(1) >= n_out &&
+                  m.stride(0) % 8 == 0 && (reinterpret_cast<uintptr_t>(m.data_ptr()) & 7) == 0 &&
+                  m.size(0) * p.seg[i].k >= p.seg[i].row1 - p.seg[i].row0,
+                  "amax_src[i] must be 8-byte aligned uint8 [parents, >= n_out] rows with a row stride multiple of 8");
+      TORCH_CHECK(p.ld_amax == 0 || p.ld_amax == m.stride(0), "all argmax views must share the row stride");
+      p.ld_amax = (int)m.stride(0);
+      p.amax[i] = reinterpret_cast<const uint8_t*>(m.data_ptr());
+      route = true;
+    }
     if (h.has_value() && h->defined()) {
       TORCH_CHECK(h->scalar_type() == at::kBFloat16 && h->dim() == 2 && h->stride(1) == 1 && h->size(0) >= p.rows &&
                   h->size(1) >= n_out && h->stride(0) % 8 == 0 && (reinterpret_cast<uintptr_t>(h->data_ptr()) & 15) == 0);
@@ -337,13 +398,8 @@ void sage_bwd_dw(const c10::optional<at::Tensor>& dz, const c10::optional<at::Te
   const int splits = (p.rows + rps - 1) / rps;
   p.lbo = 8192; p.sbo = 1024; p.kadv = 2048;
   const size_t smem = 1024 + (size_t)kDwStages * kDwStageBytes + 512 + 2 * kDwStages * 8;
-  static bool attr_done = false;
-  if (!attr_done) {
-    C10_CUDA_CHECK(cudaFuncSetAttribute(sage_bwd_dw_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_done = true;
-  }
-  sage_bwd_dw_kernel<<<blocks * splits, kDwThreads, smem, at::cuda::getCurrentCUDAStream()>>>(p);
-  C10_CUDA_KERNEL_LAUNCH_CHECK();
+  if (route) launch_dw<true>(p, blocks * splits, smem);
+  else launch_dw<false>(p, blocks * splits, smem);
 }
 
 // ------------------------------------------------------------------------------------------------

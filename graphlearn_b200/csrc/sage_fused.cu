@@ -29,8 +29,10 @@
 // The rows never round-trip through HBM ("agg(X).W" instead of materialising [B*k, D]).
 //
 // Math parity: EgoSAGEConv (graphlearn/python/nn/tf/layers/ego_sage_conv.py:71-106):
-// agg in {mean,sum} over neighbor.reshape(-1,k,d), out = W.[x || agg]; 'gcn' = mean over {x} U nbrs
-// then W.  Loss parity: graphlearn/python/nn/tf/loss.py (softmax cross entropy).
+// agg in {mean,sum,max} over neighbor.reshape(-1,k,d), out = W.[x || agg]; 'gcn' = mean over {x} U nbrs
+// then W.  Max is its own instantiation (AGG = kAggMax): the gather warps fold rows with a strict '>' in ascending
+// neighbour order and can record, per destination row and column, the first neighbour j holding the maximum (the
+// argmax bytes the backward routes the gradient with).  Loss parity: graphlearn/python/nn/tf/loss.py (softmax CE).
 #include <torch/extension.h>
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
@@ -56,7 +58,10 @@ constexpr int kMaxSegs = 4;
 constexpr int kScrCap = 64;                        // row pointers per gather warp (private scratch): rows_per_item * (k + 1) <= 64
 constexpr size_t kSmemLimit = 232448;
 
-enum SageMode : int { kConcatMean = 0, kConcatSum = 1, kGcnMean = 2 };
+enum SageMode : int { kConcatMean = 0, kConcatSum = 1, kGcnMean = 2, kConcatMax = 3 };
+// aggregation of an instantiation: kAggSum serves mean, sum and (sampled mode) gcn, whose scales are runtime factors;
+// kAggMax the max; kAggGcn the gcn mean of the CSR mode, which also loads the self row
+enum SageAgg : int { kAggSum = 0, kAggMax = 1, kAggGcn = 2 };
 
 struct SageSeg {
   const int64_t* self_vids;   // [M] or null (identity: self_base + m)
@@ -108,7 +113,35 @@ struct SageParams {
   const int* hub_cptr;
   const float* hub_part;
   int hub_stride;
+  // max launches: argmax output of segment s (or null), uint8 [M_s, amax_ld], column c = the first j in [0, k) whose
+  // neighbour row holds the maximum of column c (kept after the fields above so that their offsets do not move)
+  uint8_t* amax[kMaxSegs];
+  int amax_ld;
 };
+
+// max aggregation: fold one neighbour chunk into the running column maxima
+template <int DT, int VEC>
+__device__ __forceinline__ void max_into(const Chunk<DT>& c, float (&a)[VEC]) {
+  float x[VEC];
+  c.get(x);
+#pragma unroll
+  for (int i = 0; i < VEC; ++i) a[i] = fmaxf(a[i], x[i]);
+}
+
+// ... and record the neighbour index j of each new maximum: one byte per column, four to a register.  A strict '>'
+// over ascending j keeps the FIRST maximal neighbour (torch.argmax).
+template <int DT, int VEC>
+__device__ __forceinline__ void max_into(const Chunk<DT>& c, float (&a)[VEC], uint32_t (&ix)[2], uint32_t j) {
+  float x[VEC];
+  c.get(x);
+#pragma unroll
+  for (int i = 0; i < VEC; ++i) {
+    if (x[i] > a[i]) {
+      a[i] = x[i];
+      ix[i >> 2] = (ix[i >> 2] & ~(0xFFu << (8 * (i & 3)))) | (j << (8 * (i & 3)));
+    }
+  }
+}
 
 // write VEC consecutive K elements of tile row r starting at K column kcol (multiple of VEC)
 template <int VEC>
@@ -304,8 +337,10 @@ __device__ __forceinline__ void write_item_ptrs(const SageParams& p, const TileC
 // adjacency is walked in rounds of kScrCap ids: ids -> row pointers (vid_ptr) in the warp's scratch -> U-batched row
 // loads.  The id range of the NEXT item is prefetched at the top of an item and its first round of ids right after
 // the current row loads.  Hub rows (hub_map >= 0) sum the fp32 partial rows of their adjacency chunks instead.
+// AGG = kAggMax takes the column max (lane groups combined with shuffles, 0 for degree 0; hub rows the max of their
+// chunks' partial maxima); kAggGcn loads the self row as well and writes (x_self + sum) / (deg + 1).
 // ------------------------------------------------------------------------------------------------
-template <int U, int DT>
+template <int U, int DT, int AGG>
 __device__ __forceinline__ void sage_csr_gather(const SageParams& p, uint8_t* sA, uint32_t a_buf_bytes, uint64_t* bars,
                                                 const char** scr, int tile_first, int tile_stride, int gw, int lane) {
   constexpr int VEC = Chunk<DT>::kVec;
@@ -322,7 +357,9 @@ __device__ __forceinline__ void sage_csr_gather(const SageParams& p, uint8_t* sA
   gg.n_slices = lanes_row > 32 ? lanes_row >> 5 : 1;
   gg.lig = lane & (lpr - 1);
   gg.tile_first = tile_first; gg.tile_stride = tile_stride;
+  constexpr bool kMax = AGG == kAggMax, kGcn = AGG == kAggGcn;
   const bool has_self = p.kp_self > 0, has_nbr = p.kp_nbr > 0;
+  const bool need_self = has_self || kGcn;              // gcn: the self row joins the mean (kp_self = 0)
   const uint32_t nbr_row_bytes = (uint32_t)p.tnbr.stride * kEsz, self_row_bytes = (uint32_t)p.tself.stride * kEsz;
   const int soff_self = fp8_scale_offset(d_self), soff_nbr = fp8_scale_offset(d_nbr);
   const int n_tiles_cta = (p.total_tiles - tile_first + tile_stride - 1) / tile_stride;
@@ -370,8 +407,8 @@ __device__ __forceinline__ void sage_csr_gather(const SageParams& p, uint8_t* sA
     const int f0 = chunk * VEC;
     float acc[VEC], sv[VEC];
 #pragma unroll
-    for (int i = 0; i < VEC; ++i) { acc[i] = 0.f; sv[i] = 0.f; }
-    const bool self_ld = has_self && grp == 0 && f0 < d_self;
+    for (int i = 0; i < VEC; ++i) { acc[i] = kMax ? -INFINITY : 0.f; sv[i] = 0.f; }
+    const bool self_ld = need_self && grp == 0 && f0 < d_self;
     Chunk<DT> sraw;
     if (self_ld)
       load_chunk<DT>(sraw, vid_ptr(p.tself, sg.self_vids ? __ldg(sg.self_vids + m) : sg.self_base + m, p.wshift_self,
@@ -384,7 +421,12 @@ __device__ __forceinline__ void sage_csr_gather(const SageParams& p, uint8_t* sA
 #pragma unroll
           for (int q = 0; q < VEC / 4; ++q) {
             const float4 v = __ldcg(src + q);
-            acc[4 * q] += v.x; acc[4 * q + 1] += v.y; acc[4 * q + 2] += v.z; acc[4 * q + 3] += v.w;
+            if constexpr (kMax) {
+              acc[4 * q] = fmaxf(acc[4 * q], v.x); acc[4 * q + 1] = fmaxf(acc[4 * q + 1], v.y);
+              acc[4 * q + 2] = fmaxf(acc[4 * q + 2], v.z); acc[4 * q + 3] = fmaxf(acc[4 * q + 3], v.w);
+            } else {
+              acc[4 * q] += v.x; acc[4 * q + 1] += v.y; acc[4 * q + 2] += v.z; acc[4 * q + 3] += v.w;
+            }
           }
         }
       }
@@ -404,24 +446,39 @@ __device__ __forceinline__ void sage_csr_gather(const SageParams& p, uint8_t* sA
 #pragma unroll
             for (int u = 0; u < U; ++u) load_chunk<DT>(raw[u], scr[j + u * ngrp], chunk, soff_nbr);
 #pragma unroll
-            for (int u = 0; u < U; ++u) raw[u].add_to(acc);
+            for (int u = 0; u < U; ++u) {
+              if constexpr (kMax) max_into<DT>(raw[u], acc);
+              else raw[u].add_to(acc);
+            }
           }
           if (j < n) {
             Chunk<DT> raw[U];
 #pragma unroll
             for (int u = 0; u < U; ++u) load_chunk<DT>(raw[u], scr[j + u * ngrp < n ? j + u * ngrp : j], chunk, soff_nbr);
 #pragma unroll
-            for (int u = 0; u < U; ++u)
-              if (j + u * ngrp < n) raw[u].add_to(acc);
+            for (int u = 0; u < U; ++u) {
+              if (j + u * ngrp < n) {
+                if constexpr (kMax) max_into<DT>(raw[u], acc);
+                else raw[u].add_to(acc);
+              }
+            }
           }
         }
       }
     }
     if (nvalid && has_nbr && nhub < 0) fetch_ids(nb, ne, ids);
 #pragma unroll
-    for (int o = lpr; o < 32; o <<= 1)                  // sum the lane groups' shares of the row
+    for (int o = lpr; o < 32; o <<= 1)                  // combine the lane groups' shares of the row
 #pragma unroll
-      for (int i = 0; i < VEC; ++i) acc[i] += __shfl_xor_sync(0xffffffffu, acc[i], o);
+      for (int i = 0; i < VEC; ++i) {
+        const float v = __shfl_xor_sync(0xffffffffu, acc[i], o);
+        acc[i] = kMax ? fmaxf(acc[i], v) : acc[i] + v;
+      }
+    if constexpr (kMax) {
+      if (e_end == e_beg)                               // degree 0: zero aggregate
+#pragma unroll
+        for (int i = 0; i < VEC; ++i) acc[i] = 0.f;
+    }
     if (self_ld) sraw.add_to(sv);
     if (f0 + VEC > d_self || f0 + VEC > d_nbr) {
 #pragma unroll
@@ -437,9 +494,15 @@ __device__ __forceinline__ void sage_csr_gather(const SageParams& p, uint8_t* sA
       if (has_self) put_chunk<VEC>(sAt, nullptr, rg, f0, sv);
       if (has_nbr) {
         const int64_t deg = e_end - e_beg;              // degree 0: zero aggregate
-        const float scale = p.mode == kConcatMean ? (deg > 0 ? 1.f / (float)deg : 0.f) : 1.f;
+        if constexpr (kGcn) {
+          const float scale = 1.f / (float)(deg + 1);
 #pragma unroll
-        for (int i = 0; i < VEC; ++i) acc[i] *= scale;
+          for (int i = 0; i < VEC; ++i) acc[i] = (acc[i] + sv[i]) * scale;
+        } else {
+          const float scale = p.mode == kConcatMean ? (deg > 0 ? 1.f / (float)deg : 0.f) : 1.f;
+#pragma unroll
+          for (int i = 0; i < VEC; ++i) acc[i] *= scale;
+        }
         put_chunk<VEC>(sAt, nullptr, rg, p.kp_self + f0, acc);
       }
     }
@@ -459,8 +522,9 @@ __device__ __forceinline__ void sage_csr_gather(const SageParams& p, uint8_t* sA
 // hundred edges (static per CSR); one warp per (chunk, 512-byte slice) sums the chunk's neighbour rows in fp32 into
 // part[chunk, 0 .. kp).  The layer launch then reads a hub row's few partial rows instead of its neighbours, so a row of
 // 50 000 neighbours is spread over hundreds of warps instead of stalling one gather warp - and with it, through the
-// double-buffered A tile, its whole CTA.  Fixed chunking and summation order: the result is deterministic.
-template <int U, int DT>
+// double-buffered A tile, its whole CTA.  Fixed chunking and summation order: the result is deterministic.  MAX: the
+// chunk's column maxima instead of sums (a chunk is never empty).
+template <int U, int DT, bool MAX>
 __global__ void __launch_bounds__(256) sage_hub_partial_kernel(const __grid_constant__ TableView t, int wshift, const int64_t* __restrict__ indices,
                                                                const int64_t* __restrict__ chunks, int n_chunks, int kp,
                                                                float* __restrict__ part, const char* zero_row) {
@@ -484,7 +548,7 @@ __global__ void __launch_bounds__(256) sage_hub_partial_kernel(const __grid_cons
   const int soff = fp8_scale_offset(t.dim);
   float acc[VEC];
 #pragma unroll
-  for (int i = 0; i < VEC; ++i) acc[i] = 0.f;
+  for (int i = 0; i < VEC; ++i) acc[i] = MAX ? -INFINITY : 0.f;
   if (f0 < t.dim) {
     for (int j = grp; j < cnt; j += U * ngrp) {
       const char* ptr[U];
@@ -497,14 +561,23 @@ __global__ void __launch_bounds__(256) sage_hub_partial_kernel(const __grid_cons
 #pragma unroll
       for (int u = 0; u < U; ++u) load_chunk<DT>(raw[u], ptr[u], chunk, soff);
 #pragma unroll
-      for (int u = 0; u < U; ++u) raw[u].add_to(acc);
+      for (int u = 0; u < U; ++u) {
+        if constexpr (MAX) {
+          if (j + u * ngrp < cnt) max_into<DT>(raw[u], acc);    // (the zero row of a masked load is no candidate)
+        } else {
+          raw[u].add_to(acc);
+        }
+      }
     }
   }
 #pragma unroll
   for (int o = 1; o < 32; o <<= 1) {
     if (o < lpr) continue;                              // (warp-uniform)
 #pragma unroll
-    for (int i = 0; i < VEC; ++i) acc[i] += __shfl_xor_sync(0xffffffffu, acc[i], o);
+    for (int i = 0; i < VEC; ++i) {
+      const float v = __shfl_xor_sync(0xffffffffu, acc[i], o);
+      acc[i] = MAX ? fmaxf(acc[i], v) : acc[i] + v;
+    }
   }
   if (grp == 0) {
     float4* dst = reinterpret_cast<float4*>(part + (size_t)c * kp + f0);
@@ -518,13 +591,14 @@ __global__ void __launch_bounds__(256) sage_hub_partial_kernel(const __grid_cons
 // U  = neighbour row loads kept in flight per lane (one batch)
 // DT = storage dtype of the self AND neighbour tables (0 fp32, 1 bf16)
 // CSR = neighbour source: fixed-k id lists of the segments (false) or CSR rows of any length (true, sage_csr_gather)
+// AGG = SageAgg of the neighbour reduction
 //
 // Gather decomposition: a row needs LPR = kp / VEC lanes (16-byte chunk per lane); when LPR < 32 a
 // warp processes 32/LPR rows side by side (sub-warp groups), when LPR > 32 the row is cut into
 // 32-lane slices.  Per item a lane group issues ALL self + neighbour chunk loads of a batch
 // unconditionally (masked lanes read a zero row), reduces in fp32 and writes bf16 into the SW128
 // A tile.
-template <int U, int DT, bool CSR = false>
+template <int U, int DT, bool CSR, int AGG>
 __global__ void __launch_bounds__(kThreads, 1) sage_persist_kernel(const __grid_constant__ SageParams p) {
   if (p.dbg && threadIdx.x == 0) {
     unsigned long long gt; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt));
@@ -620,11 +694,12 @@ __global__ void __launch_bounds__(kThreads, 1) sage_persist_kernel(const __grid_
     gmma::mbar_wait(bars + kBarW, 0);
     GLB_DBG(1);
   } else if constexpr (CSR) {
-    sage_csr_gather<U, DT>(p, sA, a_buf_bytes, bars, sScr + (warp - kGatherWarp0) * kScrCap, tile_first, tile_stride,
+    sage_csr_gather<U, DT, AGG>(p, sA, a_buf_bytes, bars, sScr + (warp - kGatherWarp0) * kScrCap, tile_first, tile_stride,
                            warp - kGatherWarp0, lane);
   } else {
     // =================================================================== gather warps
     constexpr int VEC = Chunk<DT>::kVec;
+    constexpr bool kMax = AGG == kAggMax;
     const int gw = warp - kGatherWarp0;
     const int kp = p.kp_nbr > 0 ? p.kp_nbr : p.kp_self;
     const int d_self = p.tself.dim, d_nbr = p.tnbr.dim;
@@ -694,6 +769,7 @@ __global__ void __launch_bounds__(kThreads, 1) sage_persist_kernel(const __grid_
       const int chunk = gg.lig + 32 * sl;                 // this lane's 16-byte chunk of the row
       const int f0 = chunk * VEC;                         // first feature of the chunk
       float acc[VEC], sv[VEC];
+      uint32_t ix[2] = {0u, 0u};                          // (max) argmax bytes of the chunk's columns
 #pragma unroll
       for (int i = 0; i < VEC; ++i) { acc[i] = 0.f; sv[i] = 0.f; }
       if (row_ok) {
@@ -704,21 +780,33 @@ __global__ void __launch_bounds__(kThreads, 1) sage_persist_kernel(const __grid_
         Chunk<DT> sraw;
         if (self_ld) load_chunk<DT>(sraw, ptrs[k], chunk, soff_self);
         if (has_nbr && f0 < d_nbr) {
+          if constexpr (kMax) {                           // k = 0 keeps the zero aggregate
+            if (k > 0)
+#pragma unroll
+              for (int i = 0; i < VEC; ++i) acc[i] = -INFINITY;
+          }
           int j0 = 0;
           for (; j0 + U <= k; j0 += U) {                  // full batches: U unconditional loads, then U adds
             Chunk<DT> raw[U];
 #pragma unroll
             for (int u = 0; u < U; ++u) load_chunk<DT>(raw[u], ptrs[j0 + u], chunk, soff_nbr);
 #pragma unroll
-            for (int u = 0; u < U; ++u) raw[u].add_to(acc);
+            for (int u = 0; u < U; ++u) {                 // (max: ascending j, so the first maximal row wins)
+              if constexpr (kMax) max_into<DT>(raw[u], acc, ix, (uint32_t)(j0 + u));
+              else raw[u].add_to(acc);
+            }
           }
           if (j0 < k) {                                   // remainder batch (k % U rows)
             Chunk<DT> raw[U];
 #pragma unroll
             for (int u = 0; u < U; ++u) load_chunk<DT>(raw[u], ptrs[j0 + u < k ? j0 + u : k - 1], chunk, soff_nbr);
 #pragma unroll
-            for (int u = 0; u < U; ++u)
-              if (j0 + u < k) raw[u].add_to(acc);
+            for (int u = 0; u < U; ++u) {
+              if (j0 + u < k) {
+                if constexpr (kMax) max_into<DT>(raw[u], acc, ix, (uint32_t)(j0 + u));
+                else raw[u].add_to(acc);
+              }
+            }
           }
         }
         if (self_ld) sraw.add_to(sv);
@@ -745,6 +833,14 @@ __global__ void __launch_bounds__(kThreads, 1) sage_persist_kernel(const __grid_
 #pragma unroll
           for (int i = 0; i < VEC; ++i) acc[i] = (acc[i] + (p.mode == kGcnMean ? sv[i] : 0.f)) * scale;
           put_chunk<VEC>(sAt, a_row, r, p.kp_self + f0, acc);
+        }
+        if constexpr (kMax) {
+          uint8_t* am = p.amax[cur.s];
+          if (am != nullptr && img == 0 && has_nbr && f0 < d_nbr) {
+            uint8_t* dst = am + (size_t)m * p.amax_ld + f0;
+            if constexpr (VEC == 8) *reinterpret_cast<uint2*>(dst) = make_uint2(ix[0], ix[1]);
+            else *reinterpret_cast<uint32_t*>(dst) = ix[0];
+          }
         }
       }
       if (!nvalid || nit != it) {                         // last item of this warp in tile `it`
@@ -873,14 +969,14 @@ static void plan_tiles(SageParams& p) {
   p.total_tiles = tiles;
 }
 
-template <int U, int DT, bool CSR>
+template <int U, int DT, bool CSR, int AGG>
 static void launch_one(const SageParams& p, unsigned grid, size_t smem, cudaStream_t stream) {
   static bool attr_done = false;
   if (!attr_done) {
-    C10_CUDA_CHECK(cudaFuncSetAttribute(sage_persist_kernel<U, DT, CSR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemLimit));
+    C10_CUDA_CHECK(cudaFuncSetAttribute(sage_persist_kernel<U, DT, CSR, AGG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemLimit));
     attr_done = true;
   }
-  sage_persist_kernel<U, DT, CSR><<<grid, kThreads, smem, stream>>>(p);
+  sage_persist_kernel<U, DT, CSR, AGG><<<grid, kThreads, smem, stream>>>(p);
 }
 
 // row loads in flight per lane of the CSR mode (one instantiation per table dtype)
@@ -892,12 +988,17 @@ static void launch_persist(SageParams& p, size_t smem, cudaStream_t stream, bool
   int kmax = 1;
   for (int s = 0; s < p.nseg; ++s) kmax = std::max(kmax, p.seg[s].k);
   const int dt = p.tnbr.dtype;
-#define LAUNCH_DT3(UU, CC) do { if (dt == 2) launch_one<UU, 2, CC>(p, grid, smem, stream); \
-                                else if (dt == 0) launch_one<UU, 0, CC>(p, grid, smem, stream); \
-                                else launch_one<UU, 1, CC>(p, grid, smem, stream); } while (0)
+#define LAUNCH_DT3(UU, CC, AA) do { if (dt == 2) launch_one<UU, 2, CC, AA>(p, grid, smem, stream); \
+                                    else if (dt == 0) launch_one<UU, 0, CC, AA>(p, grid, smem, stream); \
+                                    else launch_one<UU, 1, CC, AA>(p, grid, smem, stream); } while (0)
   const int u = kmax <= 4 ? 4 : (kmax % 5 == 0 || kmax > 12) ? 5 : 6;
-  if (csr) LAUNCH_DT3(kCsrU, true);
-  else if (u == 4) LAUNCH_DT3(4, false); else if (u == 5) LAUNCH_DT3(5, false); else LAUNCH_DT3(6, false);
+  if (csr) {
+    if (p.mode == kConcatMax) LAUNCH_DT3(kCsrU, true, kAggMax);
+    else if (p.mode == kGcnMean) LAUNCH_DT3(kCsrU, true, kAggGcn);
+    else LAUNCH_DT3(kCsrU, true, kAggSum);
+  } else if (p.mode == kConcatMax) {
+    if (u == 4) LAUNCH_DT3(4, false, kAggMax); else if (u == 5) LAUNCH_DT3(5, false, kAggMax); else LAUNCH_DT3(6, false, kAggMax);
+  } else if (u == 4) LAUNCH_DT3(4, false, kAggSum); else if (u == 5) LAUNCH_DT3(5, false, kAggSum); else LAUNCH_DT3(6, false, kAggSum);
 #undef LAUNCH_DT3
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
@@ -959,6 +1060,8 @@ static void set_seg_out(SageParams& p, SageSeg& sg, const at::Tensor& out, int64
 // a_saves[i] ([M_i, K_total] bf16, the [self || agg] rows for the backward pass).
 // ce = optional fused softmax cross-entropy on the output rows of segment 0:
 //   [labels_table(int64), seeds(int64)|undefined, loss(fp32 >=1), dlogits(bf16 [M, stride]), dbias(fp32)|undefined]
+// amax = [] or, for a max launch, one optional uint8 [M_i, >= d_nbr rounded up to 8] view per segment (a shared row
+// stride, a multiple of 8): column c of row m receives the first neighbour j in [0, k_i) holding the maximum of column c
 void sage_fused_multi(const at::Tensor& tself_desc, const at::Tensor& tnbr_desc,
                       const std::vector<c10::optional<at::Tensor>>& self_vids,
                       const std::vector<c10::optional<at::Tensor>>& nbr_vids,
@@ -967,8 +1070,10 @@ void sage_fused_multi(const at::Tensor& tself_desc, const at::Tensor& tnbr_desc,
                       const std::vector<at::Tensor>& outs, const std::vector<c10::optional<at::Tensor>>& a_saves,
                       int64_t mode, const at::Tensor& w_img, const c10::optional<at::Tensor>& bias, int64_t N,
                       int64_t n_out, bool relu, bool out_bf16,
-                      const std::vector<c10::optional<at::Tensor>>& ce, int64_t ce_world, int64_t n_imgs) {
+                      const std::vector<c10::optional<at::Tensor>>& ce, int64_t ce_world, int64_t n_imgs,
+                      const std::vector<c10::optional<at::Tensor>>& amax) {
   TORCH_CHECK(w_img.is_cuda() && w_img.scalar_type() == at::kBFloat16, "w_img must be CUDA bf16");
+  TORCH_CHECK(mode >= kConcatMean && mode <= kConcatMax, "unknown aggregation mode ", mode);
   c10::cuda::CUDAGuard guard(w_img.device());
   const int nseg = (int)Ms.size();
   TORCH_CHECK(nseg >= 1 && nseg <= kMaxSegs, "1..", kMaxSegs, " segments per launch");
@@ -1009,6 +1114,20 @@ void sage_fused_multi(const at::Tensor& tself_desc, const at::Tensor& tnbr_desc,
       TORCH_CHECK(a.scalar_type() == at::kBFloat16 && a.dim() == 2 && a.size(0) == Ms[s] && a.size(1) == k_total &&
                   a.stride(1) == 1 && a.stride(0) == k_total, "a_saves[i] must be a row-contiguous bf16 [M_i, K_total] view");
       sg.a_save = reinterpret_cast<__nv_bfloat16*>(a.data_ptr());
+    }
+  }
+  if (!amax.empty()) {
+    TORCH_CHECK(mode == kConcatMax && (int)amax.size() == nseg, "amax needs a max launch and one entry per segment");
+    for (int s = 0; s < nseg; ++s) {
+      if (!(amax[s].has_value() && amax[s]->defined())) continue;
+      const at::Tensor& a = *amax[s];
+      TORCH_CHECK(a.is_cuda() && a.scalar_type() == at::kByte && a.dim() == 2 && a.size(0) == Ms[s] && a.stride(1) == 1 &&
+                  a.size(1) >= (p.tnbr.dim + 7) / 8 * 8 && a.stride(0) % 8 == 0 && (reinterpret_cast<uintptr_t>(a.data_ptr()) & 7) == 0,
+                  "amax[i] must be an 8-byte aligned uint8 [M_i, >= d_nbr rounded up to 8] view, row stride a multiple of 8");
+      TORCH_CHECK(ks[s] <= 256, "amax holds neighbour indices below 256");
+      TORCH_CHECK(p.amax_ld == 0 || p.amax_ld == a.stride(0), "all amax views must share the row stride");
+      p.amax_ld = (int)a.stride(0);
+      p.amax[s] = reinterpret_cast<uint8_t*>(a.data_ptr());
     }
   }
   if (p.out_stride < 0) p.out_stride = n_out;
@@ -1055,7 +1174,7 @@ void sage_fused_csr(const at::Tensor& tself_desc, const at::Tensor& tnbr_desc, c
                     int64_t N, int64_t n_out, bool relu, bool out_bf16, int64_t n_imgs, int64_t plan_deg) {
   TORCH_CHECK(w_img.is_cuda() && w_img.scalar_type() == at::kBFloat16, "w_img must be CUDA bf16");
   c10::cuda::CUDAGuard guard(w_img.device());
-  TORCH_CHECK(mode == kConcatMean || mode == kConcatSum, "CSR mode supports mean / sum aggregation");
+  TORCH_CHECK(mode >= kConcatMean && mode <= kConcatMax, "unknown aggregation mode ", mode);
   const int64_t M = self_vids.numel();
   check_cuda_i64(self_vids, "self_vids");
   check_cuda_i64(csr_indptr, "csr_indptr");
@@ -1100,12 +1219,14 @@ void sage_fused_csr(const at::Tensor& tself_desc, const at::Tensor& tnbr_desc, c
       const unsigned grid = (unsigned)((warps * 32 + 255) / 256);
       const int64_t* ch = chunks.data_ptr<int64_t>();
       float* pt = part.data_ptr<float>();
-      if (p.tnbr.dtype == 0)
-        sage_hub_partial_kernel<kCsrU, 0><<<grid, 256, 0, stream>>>(p.tnbr, p.wshift_nbr, p.csr_indices, ch, (int)n_chunks, p.kp_nbr, pt, p.zero_row);
-      else if (p.tnbr.dtype == 1)
-        sage_hub_partial_kernel<kCsrU, 1><<<grid, 256, 0, stream>>>(p.tnbr, p.wshift_nbr, p.csr_indices, ch, (int)n_chunks, p.kp_nbr, pt, p.zero_row);
-      else
-        sage_hub_partial_kernel<kCsrU, 2><<<grid, 256, 0, stream>>>(p.tnbr, p.wshift_nbr, p.csr_indices, ch, (int)n_chunks, p.kp_nbr, pt, p.zero_row);
+      // max: partial maxima; mean, sum and gcn: partial sums
+#define HUB_LAUNCH(DT, MX) sage_hub_partial_kernel<kCsrU, DT, MX><<<grid, 256, 0, stream>>>( \
+          p.tnbr, p.wshift_nbr, p.csr_indices, ch, (int)n_chunks, p.kp_nbr, pt, p.zero_row)
+      const bool mx = mode == kConcatMax;
+      if (p.tnbr.dtype == 0) { if (mx) HUB_LAUNCH(0, true); else HUB_LAUNCH(0, false); }
+      else if (p.tnbr.dtype == 1) { if (mx) HUB_LAUNCH(1, true); else HUB_LAUNCH(1, false); }
+      else { if (mx) HUB_LAUNCH(2, true); else HUB_LAUNCH(2, false); }
+#undef HUB_LAUNCH
       C10_CUDA_KERNEL_LAUNCH_CHECK();
     }
   }
@@ -1134,7 +1255,7 @@ std::vector<at::Tensor> sage_fused_forward(const at::Tensor& tself_desc,
   if (M == 0) return {out, a_save};
   sage_fused_multi(tself_desc, tnbr_desc, {self_vids}, {nbr_vids}, {0}, {0}, {M}, {k}, {out},
                    {save_a ? c10::optional<at::Tensor>(a_save) : c10::nullopt}, mode, w_img, bias, N, n_out, relu, out_bf16,
-                   {}, 1, 1);
+                   {}, 1, 1, {});
   return {out, a_save};
 }
 
@@ -1153,7 +1274,7 @@ at::Tensor tc_linear_forward(const at::Tensor& a, const at::Tensor& w_img, const
   d[0] = 1; d[1] = K; d[2] = a.stride(0); d[3] = 1; d[4] = M; d[4 + kMaxWorld] = reinterpret_cast<int64_t>(a.data_ptr());
   at::Tensor desc = at::from_blob(d.data(), {(int64_t)d.size()}, at::kLong).clone();
   sage_fused_multi(desc, desc, {c10::nullopt}, {c10::nullopt}, {0}, {0}, {M}, {0}, {out}, {c10::nullopt}, kConcatMean, w_img, bias,
-                   N, n_out, relu, out_bf16, {}, 1, 1);
+                   N, n_out, relu, out_bf16, {}, 1, 1, {});
   return out;
 }
 

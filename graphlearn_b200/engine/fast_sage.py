@@ -1,4 +1,4 @@
-"""Hand-scheduled training step for EgoGraphSAGE (any depth, mean/sum aggregation).
+"""Hand-scheduled training step for EgoGraphSAGE (any depth; mean, sum, max or gcn aggregation).
 
 Same math as ``models.graphsage.EgoGraphSAGE`` + ``SageTrainer``'s autograd
 path, but forward and backward are an explicit, minimal kernel chain over
@@ -9,6 +9,8 @@ pre-allocated buffers (static shapes -> CUDA graph friendly):
         (multi-segment); the top layer's launch also computes softmax-CE, dlogits and the bias gradient
   for l = L..1:  dW_l = dZ_l^T A_l   split-K wgmma kernel, fp32 accumulation straight into the flat gradient buffer;
                                      for l < L, dZ_l = relu'(H_l) * (self + nbr/k rows of dA_{l+1}) is computed by its producers
+                                     (gcn above: both parts scaled by 1/(k+1); max above: the neighbour part of a column
+                                     reaches only the child that held its max, from the argmax bytes of layer l+1's forward)
                  dA_l = dZ_l W_l     [l > 1] mma.sync kernel over the layer's forward weight images
   K8    ONE kernel: peer-memory all-reduce (world > 1) + Adam + gradient zeroing + bf16 weight images of the next step
 
@@ -65,9 +67,14 @@ class SageLayer:
     db: Optional[torch.Tensor]
     below: Optional[torch.Tensor]   # table descriptor of H of the layer below; None for layer 1 (feature table, hop ids)
     fwd: tuple                      # sage_fused_multi's (self_base, nbr_base, Ms, ks, outs, a_saves)
-    # sage_bwd_dw's (seg_row0, seg_row1, self_src, nbr_src, seg_k, seg_scale, nbr_col0, dz_out) for l < L, where dZ_l is
-    # computed from dA of the layer above
-    bwd: Optional[tuple] = None
+    # max aggregation, l >= 2: uint8 [rows, in_nbr padded to 16], row m of segment i = for each neighbour-half column the
+    # first of the k neighbours holding its max, written by the forward (`amax` per-segment views) for the layer below's
+    # gradient routing; layer 1 reads the feature table, which has no gradient
+    argmax: Optional[torch.Tensor] = None
+    amax: list = None
+    # sage_bwd_dw's keyword arguments (seg_row0, seg_row1, self_src, nbr_src, seg_k, seg_scale, nbr_col0, dz_out,
+    # seg_self_scale, amax_src) for l < L, where dZ_l is computed from dA of the layer above
+    bwd: Optional[dict] = None
 
 
 class FastSageTrainer:
@@ -102,7 +109,7 @@ class FastSageTrainer:
         self.convs = list(model.convs)
         self.layers: List[SageLayer] = []
         for l, c in enumerate(self.convs, 1):
-            assert c.agg_type in ("mean", "sum"), "fast engine supports mean / sum aggregation"
+            assert c.agg_type in ("mean", "sum", "max", "gcn"), "fast engine supports mean / sum / max / gcn aggregation"
             last = l == self.L
             kt = c.weight_p.size(1)
             ns, N = sage_ops.split_images(kt, c.out_dim)
@@ -118,6 +125,9 @@ class FastSageTrainer:
             A = torch.zeros(rows, kt, dtype=torch.bfloat16, device=dev)
             dZp = torch.zeros(rows, sage_ops.pad_k(c.out_dim), dtype=torch.bfloat16, device=dev)
             dA = torch.zeros(rows, kt, dtype=torch.bfloat16, device=dev) if l > 1 else None
+            argmax = None
+            if l > 1 and c.agg_type == "max":
+                argmax = torch.zeros(rows, (c.in_nbr + 15) // 16 * 16, dtype=torch.uint8, device=dev)
             below, self_base, nbr_base = None, [0] * nseg, [0] * nseg
             if l > 1:
                 # the segments' self / neighbour rows are the contiguous row ranges of segments i / i + 1 of the layer
@@ -127,9 +137,15 @@ class FastSageTrainer:
                 below, self_base, nbr_base = local_table_desc(lo.H), lo.offs[:nseg], lo.offs[1:nseg + 1]
                 da_seg = [dA[offs[i]:offs[i + 1]] for i in range(nseg)]
                 k_nbr = self.fanouts[:nseg]
-                scale = [1.0 / k if c.agg_type == "mean" else 1.0 for k in k_nbr]
-                lo.bwd = (lo.offs[:-1], lo.offs[1:], da_seg + [None], [None] + da_seg, [1] + k_nbr, [1.0] + scale,
-                          sage_ops.padded_dims(c.in_self, c.in_nbr, c.agg_type)[0], lo.dZ if lo.dA is not None else None)
+                gcn = c.agg_type == "gcn"
+                scale = [1.0 / k if c.agg_type == "mean" else 1.0 / (k + 1) if gcn else 1.0 for k in k_nbr]
+                # gcn: the self row is one of the k + 1 rows of the mean; max: the argmax rows of the parents
+                self_scale = [1.0 / (k + 1) for k in k_nbr] + [1.0] if gcn else []
+                amax_src = [None] + [argmax[offs[i]:offs[i + 1]] for i in range(nseg)] if argmax is not None else []
+                lo.bwd = dict(seg_row0=lo.offs[:-1], seg_row1=lo.offs[1:], self_src=da_seg + [None], nbr_src=[None] + da_seg,
+                              seg_k=[1] + k_nbr, seg_scale=[1.0] + scale,
+                              nbr_col0=sage_ops.padded_dims(c.in_self, c.in_nbr, c.agg_type)[0],
+                              dz_out=lo.dZ if lo.dA is not None else None, seg_self_scale=self_scale, amax_src=amax_src)
             outs = [Hp[offs[i]:offs[i + 1], :n_out] for i in range(nseg)]
             a_saves = [A[offs[i]:offs[i + 1]] for i in range(nseg)]
             self.layers.append(SageLayer(
@@ -139,7 +155,8 @@ class FastSageTrainer:
                 Hp=Hp, H=Hp[:, :c.out_dim], A=A, dZp=dZp, dZ=dZp[:, :c.out_dim], dA=dA,
                 img=torch.zeros(kt * ns * N, dtype=torch.bfloat16, device=dev),
                 dW=c.weight_p.grad, db=c.bias.grad if c.bias is not None else None,
-                below=below, fwd=(self_base, nbr_base, self.n[:nseg], self.fanouts[:nseg], outs, a_saves)))
+                below=below, fwd=(self_base, nbr_base, self.n[:nseg], self.fanouts[:nseg], outs, a_saves),
+                argmax=argmax, amax=[] if argmax is None else [argmax[offs[i]:offs[i + 1]] for i in range(nseg)]))
         # the lists other code reads; they alias the records' tensors
         self.H = [ly.H for ly in self.layers]
         self.dA = [ly.dA for ly in self.layers]
@@ -357,7 +374,7 @@ class FastSageTrainer:
                 d, self_ids, nbr_ids = ly.below, [None] * ly.nseg, [None] * ly.nseg
             ce = [self.nodes.labels.local, seeds, self.loss, ly.dZ, ly.db] if ly.fuse_ce else []
             C.sage_fused_multi(d, d, self_ids, nbr_ids, *ly.fwd, ly.mode, ly.img, ly.conv.bias, ly.N, ly.n_out,
-                               not ly.last, not ly.last, ce, self.rt.world, ly.ns)
+                               not ly.last, not ly.last, ce, self.rt.world, ly.ns, ly.amax)
             if ly.last and not ly.fuse_ce:
                 # wide / split top layer: the loss runs as its own kernel on the (padded) logits
                 self._top_loss(seeds)
@@ -370,6 +387,7 @@ class FastSageTrainer:
         #   top layer   : dW_L = dZ_L^T A_L with the dense dZ_L written by the fused loss epilogue
         #   layer l < L : dW_l = dZ_l^T A_l where dZ_l = relu'(H_l) * (self + 1/k neighbour rows of dA_{l+1}) is
         #                 computed inside the GEMM's producer warps (never stored for l = 1); bias grads fall out
+        #                 (the scales and the argmax routing of the layer above's aggregator are in ly.bwd)
         #   dA_l = dZ_l . W_l  (l >= 2) on sage_bwd_da (mma.sync) over the layer's forward weight images
         for ly in reversed(self.layers):
             if ly.last:
@@ -377,7 +395,7 @@ class FastSageTrainer:
                 with torch.cuda.stream(sA):            # dW_L runs beside dA_L
                     C.sage_bwd_dw(ly.dZ, None, [], [], [], [], [], [], 0, None, ly.A, ly.dW, None, ly.conv.out_dim)
             else:
-                C.sage_bwd_dw(None, ly.H, *ly.bwd, ly.A, ly.dW, ly.db, ly.conv.out_dim)
+                C.sage_bwd_dw(None, ly.H, a=ly.A, dw=ly.dW, dbias=ly.db, n_out=ly.conv.out_dim, **ly.bwd)
             if ly.dA is not None:
                 # dA_l [rows, K_total] = dZ_l [rows, n_split * n_img] . W_l
                 C.sage_bwd_da(ly.dZp, ly.img, ly.N, ly.ns, ly.dA)

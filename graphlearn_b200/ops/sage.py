@@ -21,7 +21,9 @@ import torch.nn.functional as F
 from .. import config as _config
 from ..parallel.runtime import local_table_desc, native
 
-MODE = {"mean": 0, "sum": 1, "gcn": 2}
+# "max": column-wise max over the k neighbour rows (the fused trainer and the CSR mode; `sage_layer`'s autograd op
+# treats the aggregate as a sum, so it never receives "max")
+MODE = {"mean": 0, "sum": 1, "gcn": 2, "max": 3}
 _SMEM_LIMIT = 232448
 
 
@@ -44,7 +46,9 @@ def padded_dims(d_self: int, d_nbr: int, mode: str):
 
 
 def fused_supported(d_self: int, d_nbr: int, n_out: int, mode: str, k: int = 0, dtype=torch.bfloat16) -> bool:
-    if max(d_self, d_nbr) > 512 or n_out > 256:
+    """Whether the persistent kernel runs this layer shape: any of the four aggregators (gcn also loads the self row,
+    counted in the k + 1 row pointers of an item)."""
+    if mode not in MODE or max(d_self, d_nbr) > 512 or n_out > 256:
         return False
     kp_self, kp_nbr = padded_dims(d_self, d_nbr, mode)
     # a gather warp keeps the row pointers of one work item (1-4 destination rows) in a 64-entry scratch
@@ -248,7 +252,7 @@ def sage_layer_reference(weight, bias, xs, xn, k, mode="mean", relu=False):
     if mode == "gcn":
         a = (xs + xn3.sum(1)) / (k + 1)
     else:
-        agg = xn3.mean(1) if mode == "mean" else xn3.sum(1)
+        agg = xn3.mean(1) if mode == "mean" else xn3.max(1).values if mode == "max" else xn3.sum(1)
         a = torch.cat([xs, agg], 1)
     y = F.linear(a, weight.float(), None if bias is None else bias.float())
     return F.relu(y) if relu else y
@@ -273,7 +277,8 @@ def sage_layer(weight_p: torch.Tensor, bias: Optional[torch.Tensor], *, k: int, 
     # torch.uint8 = fp8 block-scaled table storage (store/shards.py): only as (table, vids) operands
     ok_dt = (torch.float32, torch.bfloat16) + ((torch.uint8,) if x_self is None and x_nbr is None else ())
     compatible = dt_self == dt_nbr and dt_self in ok_dt and (kp_s == 0 or kp_s == kp_n)
-    if use_cuda and compatible and fused_supported(d_self, d_nbr, weight_p.size(0), mode, k, dt_self):
+    # max: the fused autograd op's backward spreads the aggregate's gradient like a sum, so max takes the dense path
+    if use_cuda and compatible and mode != "max" and fused_supported(d_self, d_nbr, weight_p.size(0), mode, k, dt_self):
         return _SageFusedFn.apply(weight_p, bias, x_self, x_nbr,
                                   None if self_table is None else self_table.feat_desc, self_vids,
                                   None if nbr_table is None else nbr_table.feat_desc, nbr_vids,

@@ -68,17 +68,17 @@ for i, a in enumerate(calls[:3]):
 # dW kernel launches of one eager step, re-run as they ran
 dw_calls = []
 orig_dw = C.sage_bwd_dw
-def hook_dw(*a):
-    dw_calls.append(a)
-    return orig_dw(*a)
+def hook_dw(*a, **kw):
+    dw_calls.append((a, kw))
+    return orig_dw(*a, **kw)
 tr.C = type("P", (), {"__getattr__": lambda self, n: hook_dw if n == "sage_bwd_dw" else getattr(C, n)})()
 tr._skip_opt = True
 tr.step(torch.randint(0, nodes.n_local, (1024,), generator=g))
 torch.cuda.synchronize()
-for a in dw_calls:
+for a, kw in dw_calls:
     ts = []
     for rep in range(5):
         ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        ev0.record(); orig_dw(*a); ev1.record(); torch.cuda.synchronize()
+        ev0.record(); orig_dw(*a, **kw); ev1.record(); torch.cuda.synchronize()
         ts.append(ev0.elapsed_time(ev1) * 1e3)
-    print("dW launch rows=%d: %s us" % (a[10].size(0), ["%.1f" % x for x in ts]))
+    print("dW launch rows=%d: %s us" % ((a[10] if len(a) > 10 else kw["a"]).size(0), ["%.1f" % x for x in ts]))
