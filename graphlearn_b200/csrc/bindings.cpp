@@ -37,14 +37,15 @@ void sage_fused_multi(const at::Tensor&, const at::Tensor&, const std::vector<c1
                       const std::vector<c10::optional<at::Tensor>>&, int64_t, const at::Tensor&,
                       const c10::optional<at::Tensor>&, int64_t, int64_t, bool, bool,
                       const std::vector<c10::optional<at::Tensor>>&, int64_t, int64_t,
-                      const std::vector<c10::optional<at::Tensor>>&);
+                      const std::vector<c10::optional<at::Tensor>>&, const c10::optional<at::Tensor>&, double, int64_t,
+                      const std::vector<int64_t>&);
 void sage_fused_csr(const at::Tensor&, const at::Tensor&, const at::Tensor&, const at::Tensor&, const at::Tensor&,
                     const std::vector<at::Tensor>&, const at::Tensor&, int64_t, const at::Tensor&,
                     const c10::optional<at::Tensor>&, int64_t, int64_t, bool, bool, int64_t, int64_t);
 int sm_count();
 void sage_set_debug_trace(const c10::optional<at::Tensor>&);
 // sage_bwd.cu
-void sage_bwd_da(const at::Tensor&, const at::Tensor&, int64_t, int64_t, const at::Tensor&);
+void sage_bwd_da(const at::Tensor&, const at::Tensor&, int64_t, int64_t, const at::Tensor&, double);
 void sage_bwd_dw(const c10::optional<at::Tensor>&, const c10::optional<at::Tensor>&, const std::vector<int64_t>&,
                  const std::vector<int64_t>&, const std::vector<c10::optional<at::Tensor>>&,
                  const std::vector<c10::optional<at::Tensor>>&, const std::vector<int64_t>&, const std::vector<double>&, int64_t,
@@ -73,7 +74,7 @@ void adam_flat(const at::Tensor&, const at::Tensor&, const at::Tensor&, const at
                double, double, double, double, double);
 void adam_pack(const at::Tensor&, const at::Tensor&, const at::Tensor&, const at::Tensor&, const at::Tensor&, double, double, double,
                double, double, const c10::optional<at::Tensor>&, const at::Tensor&, const c10::optional<at::Tensor>&,
-               const c10::optional<at::Tensor>&, const c10::optional<at::Tensor>&, double, bool);
+               const c10::optional<at::Tensor>&, const c10::optional<at::Tensor>&, double, bool, const c10::optional<at::Tensor>&);
 // graph_ops.cu
 std::vector<at::Tensor> relabel(const at::Tensor&, bool);
 at::Tensor relabel_lookup(const at::Tensor&, const at::Tensor&, const at::Tensor&);
@@ -183,7 +184,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("nbr_vids"), py::arg("self_base"), py::arg("nbr_base"), py::arg("Ms"), py::arg("ks"), py::arg("outs"),
         py::arg("a_saves"), py::arg("mode"), py::arg("w_img"), py::arg("bias"), py::arg("N"), py::arg("n_out"), py::arg("relu"),
         py::arg("out_bf16"), py::arg("ce"), py::arg("ce_world"), py::arg("n_imgs"),
-        py::arg("amax") = std::vector<c10::optional<at::Tensor>>());
+        py::arg("amax") = std::vector<c10::optional<at::Tensor>>(), py::arg("drop_state") = py::none(), py::arg("drop_p") = 0.0,
+        py::arg("drop_layer") = 0, py::arg("drop_row0") = std::vector<int64_t>());
   m.def("sage_fused_csr", &glb::sage_fused_csr);
   m.def("sm_count", &glb::sm_count);
   m.def("sage_set_debug_trace", &glb::sage_set_debug_trace);
@@ -192,7 +194,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("self_src"), py::arg("nbr_src"), py::arg("seg_k"), py::arg("seg_scale"), py::arg("nbr_col0"), py::arg("dz_out"),
         py::arg("a"), py::arg("dw"), py::arg("dbias"), py::arg("n_out"), py::arg("seg_self_scale") = std::vector<double>(),
         py::arg("amax_src") = std::vector<c10::optional<at::Tensor>>());
-  m.def("sage_bwd_da", &glb::sage_bwd_da);
+  // (alpha: scale of the fp32 accumulators before the bf16 store, 1 / (1 - p) below a dropout layer)
+  m.def("sage_bwd_da", &glb::sage_bwd_da, py::arg("dz"), py::arg("w_img"), py::arg("N"), py::arg("n_imgs"), py::arg("da"),
+        py::arg("alpha") = 1.0);
   m.def("pack_weight_f32", &glb::pack_weight_f32);
   m.def("tc_linear_forward", &glb::tc_linear_forward);
   m.def("softmax_ce", &glb::softmax_ce);
@@ -208,7 +212,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("step_advance", &glb::step_advance);
   m.def("copy_i64", &glb::copy_i64);
   m.def("adam_flat", &glb::adam_flat);
-  m.def("adam_pack", &glb::adam_pack);
+  m.def("adam_pack", &glb::adam_pack, py::arg("w"), py::arg("g_store"), py::arg("m"), py::arg("v"), py::arg("step"), py::arg("lr"),
+        py::arg("beta1"), py::arg("beta2"), py::arg("eps"), py::arg("weight_decay"), py::arg("loss_out"), py::arg("mats"),
+        py::arg("ar_desc"), py::arg("ar_epochs"), py::arg("ar_error"), py::arg("ar_scale"), py::arg("stage_bf16"),
+        py::arg("drop_ctr") = py::none());
   m.def("relabel", &glb::relabel);
   m.def("relabel_lookup", &glb::relabel_lookup);
   m.def("edge_scatter", &glb::edge_scatter);

@@ -238,6 +238,7 @@ struct AdamPackParams {
   long long n_pad;
   float ar_scale;
   int rank, world, stage_bf16;
+  long long* drop_ctr;               // or null: the dropout step counter of the fused trainer, advanced once per step
 };
 
 __global__ void __launch_bounds__(128) adam_pack_kernel(const __grid_constant__ AdamPackParams p) {
@@ -246,6 +247,8 @@ __global__ void __launch_bounds__(128) adam_pack_kernel(const __grid_constant__ 
   const float bc2 = 1.f - powf(p.beta2, step);
   const float step_size = p.lr / bc1;
   const float inv_sqrt_bc2 = rsqrtf(bc2);
+  // the step's forward launches, the only readers of the counter, precede this kernel on the stream
+  if (p.drop_ctr != nullptr && blockIdx.x == 0 && threadIdx.x == 0) ++*p.drop_ctr;
   if (p.error_flag != nullptr && *p.error_flag != 0) return;          // a previous collective failed: freeze the model
   // contiguous slice of 8-element chunks per block (identical on every rank: slices are matched by block index)
   const long long chunks = p.n >> 3;
@@ -378,10 +381,12 @@ __global__ void __launch_bounds__(128) adam_pack_kernel(const __grid_constant__ 
 }
 
 // mats: CPU int64 [n_mats, 5] = (off, n_out, k_total, N, img_ptr)
+// drop_ctr: optional CUDA int64 scalar incremented by one thread (the dropout step counter of the training step)
 void adam_pack(const at::Tensor& w, const at::Tensor& g_store, const at::Tensor& m, const at::Tensor& v, const at::Tensor& step,
                double lr, double beta1, double beta2, double eps, double weight_decay, const c10::optional<at::Tensor>& loss_out,
                const at::Tensor& mats, const c10::optional<at::Tensor>& ar_desc, const c10::optional<at::Tensor>& ar_epochs,
-               const c10::optional<at::Tensor>& ar_error, double ar_scale, bool stage_bf16) {
+               const c10::optional<at::Tensor>& ar_error, double ar_scale, bool stage_bf16,
+               const c10::optional<at::Tensor>& drop_ctr) {
   TORCH_CHECK(w.is_cuda() && w.scalar_type() == at::kFloat && w.is_contiguous() && w.numel() % 8 == 0, "flat params must be padded to 8");
   TORCH_CHECK(g_store.is_cuda() && g_store.scalar_type() == at::kFloat && g_store.numel() >= w.numel() && m.numel() == w.numel() && v.numel() == w.numel());
   TORCH_CHECK(mats.device().is_cpu() && mats.scalar_type() == at::kLong && mats.dim() == 2 && mats.size(1) == 5 && mats.size(0) <= kMaxPackMats);
@@ -417,6 +422,10 @@ void adam_pack(const at::Tensor& w, const at::Tensor& g_store, const at::Tensor&
     p.error_flag = ar_error->data_ptr<int>();
     p.ar_scale = (float)ar_scale;
     p.stage_bf16 = stage_bf16 ? 1 : 0;
+  }
+  if (drop_ctr.has_value() && drop_ctr->defined()) {
+    TORCH_CHECK(drop_ctr->is_cuda() && drop_ctr->scalar_type() == at::kLong && drop_ctr->numel() == 1, "drop_ctr must be a CUDA int64 scalar");
+    p.drop_ctr = reinterpret_cast<long long*>(drop_ctr->data_ptr<int64_t>());
   }
   if (p.n == 0) return;
   // small blocks: one 8-element chunk per thread per pass, spread over every SM; the grid depends only on n, so it

@@ -419,7 +419,7 @@ constexpr int kDaCtasPerSm = 4;
 
 __global__ void __launch_bounds__(kDaThreads) sage_bwd_da_kernel(const __nv_bfloat16* __restrict__ dz, int ld_dz, int rows,
                                                                  const uint8_t* __restrict__ w_img, int N, int n_imgs,
-                                                                 __nv_bfloat16* __restrict__ da, int ld_da) {
+                                                                 __nv_bfloat16* __restrict__ da, int ld_da, float alpha) {
   extern __shared__ __align__(128) uint8_t sW[];
   const int kb = blockIdx.x, nkb = gridDim.x;
   const int R = n_imgs * N;
@@ -493,16 +493,17 @@ __global__ void __launch_bounds__(kDaThreads) sage_bwd_da_kernel(const __nv_bflo
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       const int c = kb * 64 + 8 * j + 2 * t;
-      if (ok0) *reinterpret_cast<uint32_t*>(da + (size_t)r0 * ld_da + c) = pack_bf16x2(acc[j][0], acc[j][1]);
-      if (ok1) *reinterpret_cast<uint32_t*>(da + (size_t)r1 * ld_da + c) = pack_bf16x2(acc[j][2], acc[j][3]);
+      if (ok0) *reinterpret_cast<uint32_t*>(da + (size_t)r0 * ld_da + c) = pack_bf16x2(acc[j][0] * alpha, acc[j][1] * alpha);
+      if (ok1) *reinterpret_cast<uint32_t*>(da + (size_t)r1 * ld_da + c) = pack_bf16x2(acc[j][2] * alpha, acc[j][3] * alpha);
     }
   }
 }
 
-// dA [rows, K_total] = dZ [rows, >= R] . W with W given as its n_imgs forward (K-major SW128) images of N output columns
-// each ([n_imgs][K_total / 64][N][64], zero rows beyond the real outputs), R = n_imgs * N; dZ columns [n_out, R) must be
-// zero or finite.
-void sage_bwd_da(const at::Tensor& dz, const at::Tensor& w_img, int64_t N, int64_t n_imgs, const at::Tensor& da) {
+// dA [rows, K_total] = alpha * dZ [rows, >= R] . W with W given as its n_imgs forward (K-major SW128) images of N output
+// columns each ([n_imgs][K_total / 64][N][64], zero rows beyond the real outputs), R = n_imgs * N; dZ columns [n_out, R)
+// must be zero or finite.  alpha scales the fp32 accumulators before the bf16 store (alpha = 1 is exact): 1 / (1 - p)
+// when the layer's input was dropped out with rate p, which leaves dZ itself unscaled for the weight gradient.
+void sage_bwd_da(const at::Tensor& dz, const at::Tensor& w_img, int64_t N, int64_t n_imgs, const at::Tensor& da, double alpha) {
   const int64_t R = n_imgs * N;
   TORCH_CHECK(N % 8 == 0 && N >= 8 && n_imgs >= 1 && R % 32 == 0 && R <= kDaMaxR,
               "sage_bwd_da needs n_imgs images of N output columns (N a multiple of 8), n_imgs * N a multiple of 32 in [32, ",
@@ -529,7 +530,7 @@ void sage_bwd_da(const at::Tensor& dz, const at::Tensor& w_img, int64_t N, int64
   const dim3 grid((unsigned)nkb, (unsigned)std::min<int64_t>(row_blocks, std::max<int64_t>(1, kDaCtasPerSm * sm_count() / nkb)));
   sage_bwd_da_kernel<<<grid, kDaThreads, (size_t)R * 128, at::cuda::getCurrentCUDAStream()>>>(
       bf16_ptr(dz), (int)dz.stride(0), (int)rows, reinterpret_cast<const uint8_t*>(w_img.data_ptr()), (int)N, (int)n_imgs,
-      reinterpret_cast<__nv_bfloat16*>(da.data_ptr()), (int)da.stride(0));
+      reinterpret_cast<__nv_bfloat16*>(da.data_ptr()), (int)da.stride(0), (float)alpha);
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
 

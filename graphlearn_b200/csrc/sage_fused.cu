@@ -117,6 +117,14 @@ struct SageParams {
   // neighbour row holds the maximum of column c (kept after the fields above so that their offsets do not move)
   uint8_t* amax[kMaxSegs];
   int amax_ld;
+  // inverted dropout of a hidden layer's output (sampled mode), active when drop_state != nullptr: after bias and ReLU,
+  // element (row, col) of the layer's output buffer is kept and scaled by drop_scale = 1 / (1 - p) when its 16 mask bits
+  // (dropout_bits) are >= drop_thr = round(p * 65536), and zeroed otherwise.  row = drop_row0[s] + m, col = img * N + n.
+  const unsigned long long* drop_state;   // {seed, step counter}, 16-byte aligned
+  float drop_scale;
+  uint32_t drop_thr;
+  uint32_t drop_layer;
+  int drop_row0[kMaxSegs];
 };
 
 // max aggregation: fold one neighbour chunk into the running column maxima
@@ -193,20 +201,59 @@ __device__ __forceinline__ void store_pair(const SageParams& p, const SageSeg& s
   }
 }
 
+// Dropout mask bits of row `row` of a layer's output: ONE Philox4x32-10 call (key = seed, counter = (row,
+// layer << 24 | col / 32 * 4 + col / 2 % 4, step counter low, high word)) gives the 16 bits of the eight columns
+// {32 (col / 32) + 8 w + 2 (col / 2 % 4) + e : w < 4, e < 2}: word w, low half for e = 0, high half for e = 1.  These
+// are exactly the eight columns one lane of the epilogue holds in a row of a 32-column slice, so a lane draws once per
+// row and slice and the mask does not depend on the tile schedule, the CTA or the image that computes the column.
+// (Not inlined: inlined, the Philox rounds made ptxas spill 4-40 bytes in the gather roles of several instantiations at
+// the 80-register budget; as a call they use the caller's free registers and nothing spills.)
+__device__ __noinline__ uint4 dropout_bits(const SageParams& p, uint32_t row, uint32_t col) {
+  const ulonglong2 st = *reinterpret_cast<const ulonglong2*>(p.drop_state);
+  return Philox(st.x)(row, (p.drop_layer << 24) | ((col >> 5) << 2) | ((col >> 1) & 3u), (uint32_t)st.y, (uint32_t)(st.y >> 32));
+}
+
+__device__ __forceinline__ float dropout_apply(const SageParams& p, float x, uint32_t bits16) {
+  return bits16 >= p.drop_thr ? x * p.drop_scale : 0.f;
+}
+
 // d = the m64n32 accumulator of output columns [n0, n0 + 32) of the tile; bias staged once per CTA in shared memory
 // (fp32 [N], zero beyond n_out).  Warp wq of the warpgroup holds rows 16 wq + lane / 4 and 16 wq + lane / 4 + 8.
+// row0 = the output buffer row of tile row 0 and c0 = the output column of slice column 0 (dropout only).  DROP = false
+// compiles the dropout path out.  The dropout path walks the two rows in a loop that is not unrolled (the same
+// register-budget reason as dropout_bits).
+template <bool DROP>
 __device__ __forceinline__ void sage_epilogue_slice(const SageParams& p, const SageSeg& sg, const float* sBias, const float (&d)[16],
-                                                    int m0, int rows, int n0, int wq, int lane) {
+                                                    int m0, int rows, int n0, int wq, int lane, int row0, int c0) {
   const int r0 = wq * 16 + (lane >> 2);
+  if (!(DROP && p.drop_state)) {                                   // no dropout: bias -> ReLU -> store
 #pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    const int n = n0 + 8 * j + 2 * (lane & 3);
-    const float2 b = *reinterpret_cast<const float2*>(sBias + n);
+    for (int j = 0; j < 4; ++j) {
+      const int n = n0 + 8 * j + 2 * (lane & 3);
+      const float2 b = *reinterpret_cast<const float2*>(sBias + n);
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int r = r0 + 8 * h;
-      float x0 = d[4 * j + 2 * h] + b.x, x1 = d[4 * j + 2 * h + 1] + b.y;
+      for (int h = 0; h < 2; ++h) {
+        const int r = r0 + 8 * h;
+        float x0 = d[4 * j + 2 * h] + b.x, x1 = d[4 * j + 2 * h + 1] + b.y;
+        if (p.relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
+        if (r < rows) store_pair(p, sg, m0 + r, n, x0, x1);
+      }
+    }
+    return;
+  }
+#pragma unroll 1
+  for (int h = 0; h < 2; ++h) {
+    const int r = r0 + 8 * h;
+    const uint4 u = dropout_bits(p, (uint32_t)(row0 + r), (uint32_t)(c0 + n0 + 2 * (lane & 3)));
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int n = n0 + 8 * j + 2 * (lane & 3);
+      const float2 b = *reinterpret_cast<const float2*>(sBias + n);
+      float x0 = (h ? d[4 * j + 2] : d[4 * j]) + b.x, x1 = (h ? d[4 * j + 3] : d[4 * j + 1]) + b.y;
       if (p.relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
+      const uint32_t w = j == 0 ? u.x : j == 1 ? u.y : j == 2 ? u.z : u.w;
+      x0 = dropout_apply(p, x0, w & 0xFFFFu);
+      x1 = dropout_apply(p, x1, w >> 16);
       if (r < rows) store_pair(p, sg, m0 + r, n, x0, x1);
     }
   }
@@ -598,7 +645,10 @@ __global__ void __launch_bounds__(256) sage_hub_partial_kernel(const __grid_cons
 // 32-lane slices.  Per item a lane group issues ALL self + neighbour chunk loads of a batch
 // unconditionally (masked lanes read a zero row), reduces in fp32 and writes bf16 into the SW128
 // A tile.
-template <int U, int DT, bool CSR, int AGG>
+// DROP: the launch applies dropout (sampled mode only).  A template parameter rather than only the runtime field: with
+// the dropout path compiled into every instantiation (and the step counter advanced at p = 0 too) the headline step
+// measured 1.6 % slower at p = 0.
+template <int U, int DT, bool CSR, int AGG, bool DROP>
 __global__ void __launch_bounds__(kThreads, 1) sage_persist_kernel(const __grid_constant__ SageParams p) {
   if (p.dbg && threadIdx.x == 0) {
     unsigned long long gt; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt));
@@ -673,7 +723,7 @@ __global__ void __launch_bounds__(kThreads, 1) sage_persist_kernel(const __grid_
           if (lane == 0) gmma::mbar_arrive(bars + kBarAFree + buf);
         }
         // (warp < 4 here; the mask tells the compiler so: without it the <6, bf16> instantiation spills at 80 registers)
-        if (sg.out) sage_epilogue_slice(p, sg, sBias, d, m0, rows, sl * 32, warp & 3, lane);
+        if (sg.out) sage_epilogue_slice<DROP>(p, sg, sBias, d, m0, rows, sl * 32, warp & 3, lane, p.drop_row0[s] + m0, img * p.N);
       }
       if (p.ce_labels != nullptr) {
         __threadfence_block();
@@ -969,14 +1019,14 @@ static void plan_tiles(SageParams& p) {
   p.total_tiles = tiles;
 }
 
-template <int U, int DT, bool CSR, int AGG>
+template <int U, int DT, bool CSR, int AGG, bool DROP = false>
 static void launch_one(const SageParams& p, unsigned grid, size_t smem, cudaStream_t stream) {
   static bool attr_done = false;
   if (!attr_done) {
-    C10_CUDA_CHECK(cudaFuncSetAttribute(sage_persist_kernel<U, DT, CSR, AGG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemLimit));
+    C10_CUDA_CHECK(cudaFuncSetAttribute(sage_persist_kernel<U, DT, CSR, AGG, DROP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemLimit));
     attr_done = true;
   }
-  sage_persist_kernel<U, DT, CSR, AGG><<<grid, kThreads, smem, stream>>>(p);
+  sage_persist_kernel<U, DT, CSR, AGG, DROP><<<grid, kThreads, smem, stream>>>(p);
 }
 
 // row loads in flight per lane of the CSR mode (one instantiation per table dtype)
@@ -988,17 +1038,21 @@ static void launch_persist(SageParams& p, size_t smem, cudaStream_t stream, bool
   int kmax = 1;
   for (int s = 0; s < p.nseg; ++s) kmax = std::max(kmax, p.seg[s].k);
   const int dt = p.tnbr.dtype;
-#define LAUNCH_DT3(UU, CC, AA) do { if (dt == 2) launch_one<UU, 2, CC, AA>(p, grid, smem, stream); \
-                                    else if (dt == 0) launch_one<UU, 0, CC, AA>(p, grid, smem, stream); \
-                                    else launch_one<UU, 1, CC, AA>(p, grid, smem, stream); } while (0)
+#define LAUNCH_DT3(UU, CC, AA, DD) do { if (dt == 2) launch_one<UU, 2, CC, AA, DD>(p, grid, smem, stream); \
+                                        else if (dt == 0) launch_one<UU, 0, CC, AA, DD>(p, grid, smem, stream); \
+                                        else launch_one<UU, 1, CC, AA, DD>(p, grid, smem, stream); } while (0)
+#define LAUNCH_U(AA, DD) do { if (u == 4) LAUNCH_DT3(4, false, AA, DD); else if (u == 5) LAUNCH_DT3(5, false, AA, DD); \
+                              else LAUNCH_DT3(6, false, AA, DD); } while (0)
   const int u = kmax <= 4 ? 4 : (kmax % 5 == 0 || kmax > 12) ? 5 : 6;
+  const bool drop = p.drop_state != nullptr;
   if (csr) {
-    if (p.mode == kConcatMax) LAUNCH_DT3(kCsrU, true, kAggMax);
-    else if (p.mode == kGcnMean) LAUNCH_DT3(kCsrU, true, kAggGcn);
-    else LAUNCH_DT3(kCsrU, true, kAggSum);
+    if (p.mode == kConcatMax) LAUNCH_DT3(kCsrU, true, kAggMax, false);
+    else if (p.mode == kGcnMean) LAUNCH_DT3(kCsrU, true, kAggGcn, false);
+    else LAUNCH_DT3(kCsrU, true, kAggSum, false);
   } else if (p.mode == kConcatMax) {
-    if (u == 4) LAUNCH_DT3(4, false, kAggMax); else if (u == 5) LAUNCH_DT3(5, false, kAggMax); else LAUNCH_DT3(6, false, kAggMax);
-  } else if (u == 4) LAUNCH_DT3(4, false, kAggSum); else if (u == 5) LAUNCH_DT3(5, false, kAggSum); else LAUNCH_DT3(6, false, kAggSum);
+    if (drop) LAUNCH_U(kAggMax, true); else LAUNCH_U(kAggMax, false);
+  } else if (drop) LAUNCH_U(kAggSum, true); else LAUNCH_U(kAggSum, false);
+#undef LAUNCH_U
 #undef LAUNCH_DT3
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
@@ -1062,6 +1116,9 @@ static void set_seg_out(SageParams& p, SageSeg& sg, const at::Tensor& out, int64
 //   [labels_table(int64), seeds(int64)|undefined, loss(fp32 >=1), dlogits(bf16 [M, stride]), dbias(fp32)|undefined]
 // amax = [] or, for a max launch, one optional uint8 [M_i, >= d_nbr rounded up to 8] view per segment (a shared row
 // stride, a multiple of 8): column c of row m receives the first neighbour j in [0, k_i) holding the maximum of column c
+// drop_p > 0: inverted dropout with rate drop_p after bias and ReLU (a hidden layer's training forward): the mask of
+// output element (drop_row0[i] + m, img * N + n) is a function of drop_state = {seed, step counter} (int64 [2], device),
+// drop_layer and that position only (see dropout_bits); drop_p = 0 (the default) launches exactly as before
 void sage_fused_multi(const at::Tensor& tself_desc, const at::Tensor& tnbr_desc,
                       const std::vector<c10::optional<at::Tensor>>& self_vids,
                       const std::vector<c10::optional<at::Tensor>>& nbr_vids,
@@ -1071,7 +1128,8 @@ void sage_fused_multi(const at::Tensor& tself_desc, const at::Tensor& tnbr_desc,
                       int64_t mode, const at::Tensor& w_img, const c10::optional<at::Tensor>& bias, int64_t N,
                       int64_t n_out, bool relu, bool out_bf16,
                       const std::vector<c10::optional<at::Tensor>>& ce, int64_t ce_world, int64_t n_imgs,
-                      const std::vector<c10::optional<at::Tensor>>& amax) {
+                      const std::vector<c10::optional<at::Tensor>>& amax, const c10::optional<at::Tensor>& drop_state,
+                      double drop_p, int64_t drop_layer, const std::vector<int64_t>& drop_row0) {
   TORCH_CHECK(w_img.is_cuda() && w_img.scalar_type() == at::kBFloat16, "w_img must be CUDA bf16");
   TORCH_CHECK(mode >= kConcatMean && mode <= kConcatMax, "unknown aggregation mode ", mode);
   c10::cuda::CUDAGuard guard(w_img.device());
@@ -1131,6 +1189,24 @@ void sage_fused_multi(const at::Tensor& tself_desc, const at::Tensor& tnbr_desc,
     }
   }
   if (p.out_stride < 0) p.out_stride = n_out;
+  TORCH_CHECK(drop_p >= 0.0 && drop_p < 1.0, "dropout rate must be in [0, 1), got ", drop_p);
+  if (drop_p > 0.0) {
+    TORCH_CHECK(drop_state.has_value() && drop_state->defined(), "dropout needs its {seed, counter} state");
+    const at::Tensor& st = *drop_state;
+    TORCH_CHECK(st.is_cuda() && st.scalar_type() == at::kLong && st.numel() == 2 && st.is_contiguous() &&
+                (reinterpret_cast<uintptr_t>(st.data_ptr()) & 15) == 0, "drop_state must be a 16-byte aligned CUDA int64 [2]");
+    TORCH_CHECK(ce.empty(), "dropout applies to hidden layers, not to the fused-CE top layer");
+    TORCH_CHECK((int)drop_row0.size() == nseg, "drop_row0 needs one row offset per segment");
+    TORCH_CHECK(drop_layer >= 0 && drop_layer < 256, "drop_layer must be in [0, 256)");
+    p.drop_state = reinterpret_cast<const unsigned long long*>(st.data_ptr());
+    p.drop_thr = (uint32_t)std::llround(drop_p * 65536.0);
+    p.drop_scale = (float)(1.0 / (1.0 - drop_p));
+    p.drop_layer = (uint32_t)drop_layer;
+    for (int s = 0; s < nseg; ++s) {
+      TORCH_CHECK(drop_row0[s] >= 0 && drop_row0[s] + Ms[s] <= (int64_t)INT32_MAX, "drop_row0 out of range");
+      p.drop_row0[s] = (int)drop_row0[s];
+    }
+  }
   if (!ce.empty()) {
     TORCH_CHECK(ce.size() == 5 && nseg == 1 && N <= 64, "fused CE needs one segment and n_out <= 64");
     TORCH_CHECK(p.seg[0].out != nullptr && !out_bf16, "fused CE needs the fp32 logits output (its second phase re-reads it)");
@@ -1255,7 +1331,7 @@ std::vector<at::Tensor> sage_fused_forward(const at::Tensor& tself_desc,
   if (M == 0) return {out, a_save};
   sage_fused_multi(tself_desc, tnbr_desc, {self_vids}, {nbr_vids}, {0}, {0}, {M}, {k}, {out},
                    {save_a ? c10::optional<at::Tensor>(a_save) : c10::nullopt}, mode, w_img, bias, N, n_out, relu, out_bf16,
-                   {}, 1, 1, {});
+                   {}, 1, 1, {}, c10::nullopt, 0.0, 0, {});
   return {out, a_save};
 }
 
@@ -1274,7 +1350,7 @@ at::Tensor tc_linear_forward(const at::Tensor& a, const at::Tensor& w_img, const
   d[0] = 1; d[1] = K; d[2] = a.stride(0); d[3] = 1; d[4] = M; d[4 + kMaxWorld] = reinterpret_cast<int64_t>(a.data_ptr());
   at::Tensor desc = at::from_blob(d.data(), {(int64_t)d.size()}, at::kLong).clone();
   sage_fused_multi(desc, desc, {c10::nullopt}, {c10::nullopt}, {0}, {0}, {M}, {0}, {out}, {c10::nullopt}, kConcatMean, w_img, bias,
-                   N, n_out, relu, out_bf16, {}, 1, 1, {});
+                   N, n_out, relu, out_bf16, {}, 1, 1, {}, c10::nullopt, 0.0, 0, {});
   return out;
 }
 

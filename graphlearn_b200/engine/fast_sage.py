@@ -13,6 +13,18 @@ pre-allocated buffers (static shapes -> CUDA graph friendly):
                                      reaches only the child that held its max, from the argmax bytes of layer l+1's forward)
                  dA_l = dZ_l W_l     [l > 1] mma.sync kernel over the layer's forward weight images
   K8    ONE kernel: peer-memory all-reduce (world > 1) + Adam + gradient zeroing + bf16 weight images of the next step
+        (+ the dropout step counter when p > 0)
+
+Dropout (``model.dropout = p``, read once at construction; it is part of the captured graphs): the output of every
+hidden layer l < L is ``H_l = relu(Z_l) * m / (1 - p)`` with m ~ Bernoulli(1 - p) per element, as the reference's EgoGNN
+drops each hidden hop tensor once after the activation.  A row of H_l is both a self row and a neighbour row of layer
+l + 1, and both read the same dropped value.  Neither the layer-1 input features nor the top layer (logits,
+embeddings) are dropped, and ``infer_all`` / ``evaluate`` / ``predict`` / ``embed`` never drop.  The mask is drawn in
+the forward epilogue (after bias and ReLU, before the bf16 store) and is a pure function of (dropout seed, step
+counter, layer l, row of the layer's output buffer, output column) - see ``dropout_bits`` in csrc/sage_fused.cu.  The
+seed is the sampler's per-rank seed with its own salt; the counter is advanced by ``adam_pack`` after every forward
+launch of the step.  No mask is stored: H_l > 0 exactly where m * relu'(Z_l) = 1, so the dW kernel's relu'(H_l) test
+applies the mask and ``sage_bwd_da`` of layer l + 1 applies the 1 / (1 - p).
 
 9 launches of this repo's kernels (0 library kernels) for the 2-layer flagship instead of ~60 on the autograd path.
 Layer l consumes hop pairs (i, i+1) for i in 0..L-l, exactly the EgoGNN
@@ -67,6 +79,10 @@ class SageLayer:
     db: Optional[torch.Tensor]
     below: Optional[torch.Tensor]   # table descriptor of H of the layer below; None for layer 1 (feature table, hop ids)
     fwd: tuple                      # sage_fused_multi's (self_base, nbr_base, Ms, ks, outs, a_saves)
+    # sage_fused_multi's (drop_state, drop_p, drop_layer, drop_row0): dropout of this layer's output (hidden layers with
+    # p > 0; (None, 0.0, 0, []) otherwise)
+    drop: tuple
+    da_alpha: float                 # scale of dA: 1 / (1 - p) when the layer's input H_{l-1} is dropped out, else 1
     # max aggregation, l >= 2: uint8 [rows, in_nbr padded to 16], row m of segment i = for each neighbour-half column the
     # first of the k neighbours holding its max, written by the forward (`amax` per-segment views) for the layer below's
     # gradient routing; layer 1 reads the feature table, which has no gradient
@@ -88,10 +104,18 @@ class FastSageTrainer:
         self.L = len(self.fanouts)
         assert self.L == model.num_layers
         self.B = int(batch_size)
+        self.dropout = float(getattr(model, "dropout", 0.0))
+        if not 0.0 <= self.dropout < 1.0:
+            raise ValueError("dropout must be in [0, 1), got %r" % (self.dropout,))
         self.strategy = strategy
         self.C = native()
         dev = rt.device
         self.rng = rng_ops.DeviceRng(rt, seed)
+        # dropout masks: {seed, step counter}; the seed is the sampler's per-rank seed with its own salt, the counter is
+        # advanced by adam_pack once per step (never by the sampling branch, which runs beside the forward under capture)
+        self.drop_state = torch.tensor([(self.rng.seed * 0x9E3779B1 + self.DROPOUT_SALT) % 2 ** 63, 0],
+                                       dtype=torch.int64, device=dev)
+        self._drop_ctr = self.drop_state[1:] if self.dropout > 0 else None
         self.flat_p, self.flat_g = comm_ops.flatten_module(model)
         if rt.world > 1:            # replicas start from rank 0's initialisation (what DDP does at construction)
             import torch.distributed as dist
@@ -146,6 +170,7 @@ class FastSageTrainer:
                               seg_k=[1] + k_nbr, seg_scale=[1.0] + scale,
                               nbr_col0=sage_ops.padded_dims(c.in_self, c.in_nbr, c.agg_type)[0],
                               dz_out=lo.dZ if lo.dA is not None else None, seg_self_scale=self_scale, amax_src=amax_src)
+            drop = (self.drop_state, self.dropout, l, offs[:-1]) if self.dropout > 0 and not last else (None, 0.0, 0, [])
             outs = [Hp[offs[i]:offs[i + 1], :n_out] for i in range(nseg)]
             a_saves = [A[offs[i]:offs[i + 1]] for i in range(nseg)]
             self.layers.append(SageLayer(
@@ -156,6 +181,7 @@ class FastSageTrainer:
                 img=torch.zeros(kt * ns * N, dtype=torch.bfloat16, device=dev),
                 dW=c.weight_p.grad, db=c.bias.grad if c.bias is not None else None,
                 below=below, fwd=(self_base, nbr_base, self.n[:nseg], self.fanouts[:nseg], outs, a_saves),
+                drop=drop, da_alpha=1.0 / (1.0 - self.dropout) if l > 1 else 1.0,
                 argmax=argmax, amax=[] if argmax is None else [argmax[offs[i]:offs[i + 1]] for i in range(nseg)]))
         # the lists other code reads; they alias the records' tensors
         self.H = [ly.H for ly in self.layers]
@@ -306,6 +332,7 @@ class FastSageTrainer:
 
     # ------------------------------------------------------------------ what a subclass with other roots / loss replaces
     _fuse_ce = True         # the top layer's forward launch computes softmax-CE in its epilogue when it fits
+    DROPOUT_SALT = 0x44524F50       # salt of the dropout seed ("DROP")
 
     def _fill_slot(self, slot: int, seed_ids_host: torch.Tensor):
         """write one host batch into pinned staging slot `slot` (here: B seed vids)"""
@@ -374,7 +401,7 @@ class FastSageTrainer:
                 d, self_ids, nbr_ids = ly.below, [None] * ly.nseg, [None] * ly.nseg
             ce = [self.nodes.labels.local, seeds, self.loss, ly.dZ, ly.db] if ly.fuse_ce else []
             C.sage_fused_multi(d, d, self_ids, nbr_ids, *ly.fwd, ly.mode, ly.img, ly.conv.bias, ly.N, ly.n_out,
-                               not ly.last, not ly.last, ce, self.rt.world, ly.ns, ly.amax)
+                               not ly.last, not ly.last, ce, self.rt.world, ly.ns, ly.amax, *ly.drop)
             if ly.last and not ly.fuse_ce:
                 # wide / split top layer: the loss runs as its own kernel on the (padded) logits
                 self._top_loss(seeds)
@@ -388,7 +415,8 @@ class FastSageTrainer:
         #   layer l < L : dW_l = dZ_l^T A_l where dZ_l = relu'(H_l) * (self + 1/k neighbour rows of dA_{l+1}) is
         #                 computed inside the GEMM's producer warps (never stored for l = 1); bias grads fall out
         #                 (the scales and the argmax routing of the layer above's aggregator are in ly.bwd)
-        #   dA_l = dZ_l . W_l  (l >= 2) on sage_bwd_da (mma.sync) over the layer's forward weight images
+        #   dA_l = dZ_l . W_l  (l >= 2) on sage_bwd_da (mma.sync) over the layer's forward weight images, times
+        #                 1 / (1 - p) when H_{l-1} is dropped out (dZ_l itself stays unscaled: dW_l reads it too)
         for ly in reversed(self.layers):
             if ly.last:
                 sA.wait_stream(main)
@@ -398,7 +426,7 @@ class FastSageTrainer:
                 C.sage_bwd_dw(None, ly.H, a=ly.A, dw=ly.dW, dbias=ly.db, n_out=ly.conv.out_dim, **ly.bwd)
             if ly.dA is not None:
                 # dA_l [rows, K_total] = dZ_l [rows, n_split * n_img] . W_l
-                C.sage_bwd_da(ly.dZp, ly.img, ly.N, ly.ns, ly.dA)
+                C.sage_bwd_da(ly.dZp, ly.img, ly.N, ly.ns, ly.dA, ly.da_alpha)
         # ---- join, gradient all-reduce + fused optimiser (Adam + zero grads + next step's weight images)
         main.wait_stream(sA)
         if pipe is not None:
@@ -413,11 +441,12 @@ class FastSageTrainer:
             # ONE kernel: stage grads (scaled, optionally bf16) -> cross-GPU flag barrier -> pull + reduce every peer's
             # slice in registers -> Adam -> zero grads -> next step's weight images (K8 fused with cast/scale + optimiser)
             C.adam_pack(self.flat_p, self.g_store, o.m, o.v, o.step_t, o.lr, o.betas[0], o.betas[1], o.eps, o.wd,
-                        self.loss_out, self._mats, ar.desc, ar.epochs, ar.error, 1.0 / self.rt.world, self.ar_bf16)
+                        self.loss_out, self._mats, ar.desc, ar.epochs, ar.error, 1.0 / self.rt.world, self.ar_bf16,
+                        self._drop_ctr)
         else:
             ar(self.flat_g, average=True)
             C.adam_pack(self.flat_p, self.g_store, o.m, o.v, o.step_t, o.lr, o.betas[0], o.betas[1], o.eps, o.wd,
-                        self.loss_out, self._mats, None, None, None, 1.0, False)
+                        self.loss_out, self._mats, None, None, None, 1.0, False, self._drop_ctr)
 
     def repack(self):
         """Rebuild the bf16 weight images from the fp32 master weights (after init / load_state_dict / any
@@ -591,7 +620,7 @@ class FastSageTrainer:
 
     def state_dict(self):
         return {"model": self.flat_p.clone(), "opt": self.opt.state_dict(), "rng": self.rng.state_dict(),
-                "steps": self._steps}
+                "steps": self._steps, "dropout_state": self.drop_state.cpu()}
 
     def load_state_dict(self, sd):
         self.flat_p.copy_(sd["model"])
@@ -599,3 +628,5 @@ class FastSageTrainer:
         self.opt.load_state_dict(sd["opt"])
         self.rng.load_state_dict(sd["rng"])
         self._steps = int(sd["steps"])
+        if "dropout_state" in sd:       # (checkpoints written before dropout training keep this trainer's own state)
+            self.drop_state.copy_(sd["dropout_state"])

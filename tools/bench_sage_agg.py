@@ -1,13 +1,13 @@
-"""Speed of the fused GraphSAGE engine per aggregator (mean, sum, max, gcn) on the headline workload.
+"""Speed of the fused GraphSAGE engine per aggregator (mean, sum, max, gcn) and dropout rate on the headline workload.
 
-For each aggregator it builds the `products_sage2` trainer exactly as bench.py does (gl.Graph -> GSL query ->
-FastSageTrainer.from_query, bf16 feature rows) around ``EgoGraphSAGE(..., agg_type=a)`` and reports
+For each aggregator and dropout rate it builds the `products_sage2` trainer exactly as bench.py does (gl.Graph -> GSL
+query -> FastSageTrainer.from_query, bf16 feature rows) around ``EgoGraphSAGE(..., agg_type=a, dropout=p)`` and reports
   - steps/s of the captured step (bench.time_trainer's device-timed region),
   - the device time of every kernel of one replay (torch.profiler, mean over the profiled replays),
   - ``infer_all`` in ms (CUDA events, after a warm-up call).
 The card name, power limit and max SM clock are printed in the same run.
 
-    python tools/bench_sage_agg.py [--agg mean max gcn] [--steps 1000] [--warmup 20] [--small]
+    python tools/bench_sage_agg.py [--agg mean max gcn] [--dropout 0 0.5] [--steps 1000] [--warmup 20] [--small]
 """
 import argparse
 import os
@@ -28,6 +28,7 @@ def main():
 
     ap = argparse.ArgumentParser()
     ap.add_argument("--agg", nargs="+", default=["mean", "sum", "max", "gcn"], choices=["mean", "sum", "max", "gcn"])
+    ap.add_argument("--dropout", nargs="+", type=float, default=[0.0], help="dropout rates between the layers")
     ap.add_argument("--steps", type=int, default=1000)
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--replays", type=int, default=6, help="profiled replays for the per-kernel times")
@@ -42,14 +43,15 @@ def main():
     if a.small:
         shape = dict(num_nodes=200_000, num_edges=5_000_000, feat_dim=100, num_classes=47)
     base = graphsage.EgoGraphSAGE
-    for agg in a.agg:
-        # bench.build_trainer constructs graphsage.EgoGraphSAGE(in, hidden, classes, layers): give it the aggregator
-        graphsage.EgoGraphSAGE = lambda *p, _agg=agg, **kw: base(*p, agg_type=_agg, **kw)
+    for agg, drop in [(x, q) for x in a.agg for q in a.dropout]:
+        # bench.build_trainer constructs graphsage.EgoGraphSAGE(in, hidden, classes, layers): give it the aggregator and
+        # the dropout rate
+        graphsage.EgoGraphSAGE = lambda *p, _agg=agg, _drop=drop, **kw: base(*p, agg_type=_agg, dropout=_drop, **kw)
         try:
             tr, nodes, _, _, _, g = bench.build_trainer(args, rt, shape, "bf16", 0)
         finally:
             graphsage.EgoGraphSAGE = base
-        assert all(c.agg_type == agg for c in tr.convs)
+        assert all(c.agg_type == agg for c in tr.convs) and tr.dropout == drop
         ms_dev = bench.time_trainer(args, rt, tr, nodes, a.steps)[0]
         sps = a.steps / (ms_dev / 1e3)
         # per-kernel device time of the captured step
@@ -80,8 +82,8 @@ def main():
             e1.record()
             torch.cuda.synchronize()
             t_inf.append(e0.elapsed_time(e1))
-        print("agg=%s  steps/s %.0f  (%d steps, %.1f us/step)  infer_all ms %s" %
-              (agg, sps, a.steps, ms_dev * 1e3 / a.steps, " / ".join("%.2f" % t for t in t_inf)))
+        print("agg=%s dropout=%g  steps/s %.0f  (%d steps, %.1f us/step)  infer_all ms %s" %
+              (agg, drop, sps, a.steps, ms_dev * 1e3 / a.steps, " / ".join("%.2f" % t for t in t_inf)))
         print("  kernel us per replay (mean of %d): %s" %
               (n_rep, "  ".join("%s %.1f" % (k, v / max(n_rep, 1)) for k, v in per.items())))
         del tr, nodes, g
