@@ -51,6 +51,12 @@ void sage_bwd_dw(const c10::optional<at::Tensor>&, const c10::optional<at::Tenso
                  const std::vector<c10::optional<at::Tensor>>&, const std::vector<int64_t>&, const std::vector<double>&, int64_t,
                  const c10::optional<at::Tensor>&, const at::Tensor&, const at::Tensor&, const c10::optional<at::Tensor>&, int64_t,
                  const std::vector<double>&, const std::vector<c10::optional<at::Tensor>>&);
+// sage_embed.cu
+void embed_grad_scatter(const at::Tensor&, const std::vector<int64_t>&, const std::vector<at::Tensor>&, const std::vector<at::Tensor>&,
+                        const std::vector<int64_t>&, const std::vector<double>&, const std::vector<double>&, int64_t,
+                        const std::vector<c10::optional<at::Tensor>>&, const at::Tensor&, const at::Tensor&);
+void embed_lazy_adam(const at::Tensor&, const at::Tensor&, const at::Tensor&, const at::Tensor&, const at::Tensor&,
+                     const at::Tensor&, const at::Tensor&, double, double, double, double);
 // train_ops.cu
 void softmax_ce(const at::Tensor&, const at::Tensor&, const c10::optional<at::Tensor>&, int64_t, const at::Tensor&,
                 const at::Tensor&, const c10::optional<at::Tensor>&);
@@ -197,6 +203,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   // (alpha: scale of the fp32 accumulators before the bf16 store, 1 / (1 - p) below a dropout layer)
   m.def("sage_bwd_da", &glb::sage_bwd_da, py::arg("dz"), py::arg("w_img"), py::arg("N"), py::arg("n_imgs"), py::arg("da"),
         py::arg("alpha") = 1.0);
+  m.def("embed_grad_scatter", &glb::embed_grad_scatter, py::arg("da"), py::arg("seg_row0"), py::arg("self_ids"),
+        py::arg("nbr_ids"), py::arg("seg_k"), py::arg("self_scale"), py::arg("nbr_scale"), py::arg("nbr_col0"), py::arg("amax"),
+        py::arg("grad"), py::arg("bits"));
+  m.def("embed_lazy_adam", &glb::embed_lazy_adam, py::arg("w"), py::arg("m"), py::arg("v"), py::arg("grad"), py::arg("img"),
+        py::arg("bits"), py::arg("step"), py::arg("lr"), py::arg("beta1"), py::arg("beta2"), py::arg("eps"));
   m.def("pack_weight_f32", &glb::pack_weight_f32);
   m.def("tc_linear_forward", &glb::tc_linear_forward);
   m.def("softmax_ce", &glb::softmax_ce);

@@ -26,7 +26,16 @@ seed is the sampler's per-rank seed with its own salt; the counter is advanced b
 launch of the step.  No mask is stored: H_l > 0 exactly where m * relu'(Z_l) = 1, so the dW kernel's relu'(H_l) test
 applies the mask and ``sage_bwd_da`` of layer l + 1 applies the 1 / (1 - p).
 
-9 launches of this repo's kernels (0 library kernels) for the 2-layer flagship instead of ~60 on the autograd path.
+Learned input embedding (``learn_input_embedding=True``, for node tables without float attributes): layer 1 reads a
+trainable table E ``[n_local, d]`` (d = the first layer's input width) through its bf16 image, as it reads a feature
+table otherwise.  The backward adds three launches: dW_1 also stores dZ_1 (and a max layer 1's forward its argmax bytes),
+dA_1 = dZ_1 W_1 runs on ``sage_bwd_da``, and ``embed_grad_scatter`` adds the self / neighbour halves of dA_1 (scaled like
+the layer's aggregator) into an fp32 gradient table and marks the rows read in a bitmap.  ``embed_lazy_adam`` then updates
+the touched rows only (``torch.optim.SparseAdam``'s semantics at the dense Adam's step count), rewrites their bf16 image
+rows and clears their gradient rows and bits, on a branch beside ``adam_pack``.
+
+9 launches of this repo's kernels (0 library kernels) for the 2-layer flagship instead of ~60 on the autograd path
+(12 with the learned input embedding).
 Layer l consumes hop pairs (i, i+1) for i in 0..L-l, exactly the EgoGNN
 recursion of graphlearn/python/nn/tf/model/ego_gnn.py:58-110.
 
@@ -73,7 +82,7 @@ class SageLayer:
     A: torch.Tensor                 # saved [self || agg] tiles (bf16)
     dZp: torch.Tensor               # dZ with the row padded to the K padding of the dA GEMM
     dZ: torch.Tensor
-    dA: Optional[torch.Tensor]      # None for layer 1
+    dA: Optional[torch.Tensor]      # None for layer 1, unless it reads the learned input table
     img: torch.Tensor               # bf16 weight images (rewritten by the fused Adam kernel at the end of every step)
     dW: torch.Tensor                # the weight's and the bias's views of the flat gradient buffer
     db: Optional[torch.Tensor]
@@ -85,7 +94,7 @@ class SageLayer:
     da_alpha: float                 # scale of dA: 1 / (1 - p) when the layer's input H_{l-1} is dropped out, else 1
     # max aggregation, l >= 2: uint8 [rows, in_nbr padded to 16], row m of segment i = for each neighbour-half column the
     # first of the k neighbours holding its max, written by the forward (`amax` per-segment views) for the layer below's
-    # gradient routing; layer 1 reads the feature table, which has no gradient
+    # gradient routing; layer 1 has them only when it reads the learned input table (a feature table has no gradient)
     argmax: Optional[torch.Tensor] = None
     amax: list = None
     # sage_bwd_dw's keyword arguments (seg_row0, seg_row1, self_src, nbr_src, seg_k, seg_scale, nbr_col0, dz_out,
@@ -93,10 +102,29 @@ class SageLayer:
     bwd: Optional[dict] = None
 
 
+@dataclass
+class InputEmbedding:
+    """The learned layer-1 input table E ``[n_local, d]`` of a trainer built with ``learn_input_embedding=True``: row r
+    is the node with vid ``r * world + rank``.  Layer 1 reads its bf16 image; the fp32 tables (master, Adam moments,
+    gradient) have ``dp = d`` rounded up to 8 columns, whose padding stays zero."""
+    d: int
+    table: object                   # SymmTensor: bf16 image [n_local, stride], stride by the feature tables' rules
+    desc: torch.Tensor              # its table descriptor (what layer 1 reads where a feature table's is read otherwise)
+    view: object                    # NodeTable-like (rt, feats, feat_desc, float_dim) over the image: predict / embed
+    master: torch.Tensor            # fp32 [n_local, dp]
+    m: torch.Tensor
+    v: torch.Tensor
+    grad: torch.Tensor              # fp32 [n_local, dp], scattered by embed_grad_scatter, zeroed row by row by the update
+    bits: torch.Tensor              # int32 [ceil(n_local / 32)]: rows touched by the step (cleared by the update)
+    lr: float
+    scatter: dict                   # embed_grad_scatter's per-layout arguments (seg_row0, seg_k, self_scale, nbr_scale, ...)
+
+
 class FastSageTrainer:
     def __init__(self, rt: Runtime, nodes: NodeTable, csr: CsrShard, model, fanouts: Sequence[int], batch_size: int,
                  lr: float = 3e-3, strategy: str = "random", use_cuda_graph: bool = True, allreduce: str = "peer",
-                 seed: int = 0, allreduce_dtype: str = "fp32"):
+                 seed: int = 0, allreduce_dtype: str = "fp32", learn_input_embedding: bool = False,
+                 embedding_lr: Optional[float] = None):
         self.ar_bf16 = allreduce_dtype == "bf16"      # stage the gradient exchange in bf16 (halves the NVLink bytes)
         assert rt.is_cuda, "FastSageTrainer is the CUDA engine; use SageTrainer for the portable path"
         self.rt, self.nodes, self.csr, self.model = rt, nodes, csr, model
@@ -107,6 +135,8 @@ class FastSageTrainer:
         self.dropout = float(getattr(model, "dropout", 0.0))
         if not 0.0 <= self.dropout < 1.0:
             raise ValueError("dropout must be in [0, 1), got %r" % (self.dropout,))
+        if learn_input_embedding:
+            self._check_input_embedding(rt, nodes, model, self.fanouts)
         self.strategy = strategy
         self.C = native()
         dev = rt.device
@@ -148,9 +178,10 @@ class FastSageTrainer:
             Hp = torch.zeros(rows, ns * N if last else c.out_dim, dtype=torch.float32 if last else torch.bfloat16, device=dev)
             A = torch.zeros(rows, kt, dtype=torch.bfloat16, device=dev)
             dZp = torch.zeros(rows, sage_ops.pad_k(c.out_dim), dtype=torch.bfloat16, device=dev)
-            dA = torch.zeros(rows, kt, dtype=torch.bfloat16, device=dev) if l > 1 else None
+            # (layer 1 has a dA, and a max layer 1 its argmax bytes, only when its input is the learned table)
+            dA = torch.zeros(rows, kt, dtype=torch.bfloat16, device=dev) if l > 1 or learn_input_embedding else None
             argmax = None
-            if l > 1 and c.agg_type == "max":
+            if (l > 1 or learn_input_embedding) and c.agg_type == "max":
                 argmax = torch.zeros(rows, (c.in_nbr + 15) // 16 * 16, dtype=torch.uint8, device=dev)
             below, self_base, nbr_base = None, [0] * nseg, [0] * nseg
             if l > 1:
@@ -183,6 +214,9 @@ class FastSageTrainer:
                 below=below, fwd=(self_base, nbr_base, self.n[:nseg], self.fanouts[:nseg], outs, a_saves),
                 drop=drop, da_alpha=1.0 / (1.0 - self.dropout) if l > 1 else 1.0,
                 argmax=argmax, amax=[] if argmax is None else [argmax[offs[i]:offs[i + 1]] for i in range(nseg)]))
+        self.emb: Optional[InputEmbedding] = None
+        if learn_input_embedding:
+            self.emb = self._make_input_embedding(lr if embedding_lr is None else float(embedding_lr))
         # the lists other code reads; they alias the records' tensors
         self.H = [ly.H for ly in self.layers]
         self.dA = [ly.dA for ly in self.layers]
@@ -215,6 +249,72 @@ class FastSageTrainer:
         # root traversal driving step_query (installed by from_query / a subclass), its next-epoch prefetch thread
         self._q_iter = self._q_thread = self._q_next = None
         self._inf = None                # infer_all: (CSR plan, local vids, hidden-layer tables), built on first call
+
+    # ------------------------------------------------------------------ learned input embedding
+    EMBED_SALT = 0x454D4244         # salt of the input embedding's initialisation seed ("EMBD")
+
+    @staticmethod
+    def _check_input_embedding(rt: Runtime, nodes: NodeTable, model, fanouts: Sequence[int]):
+        c = model.convs[0]
+        if nodes.float_dim > 0:
+            raise ValueError("learn_input_embedding replaces the node table's float attributes as the layer-1 input; this "
+                             "table has %d of them (concatenating attributes with a learned embedding is not supported)"
+                             % nodes.float_dim)
+        if c.in_self != c.in_nbr:
+            raise ValueError("learn_input_embedding needs the first layer's self and neighbour input widths to be equal "
+                             "(got %d and %d)" % (c.in_self, c.in_nbr))
+        _, N = sage_ops.split_images(c.weight_p.size(1), c.out_dim)
+        if c.in_self < 1 or not sage_ops.fused_supported(c.in_self, c.in_nbr, min(c.out_dim, N), c.agg_type, max(fanouts)):
+            raise ValueError("learn_input_embedding: the fused layer does not run a %d-wide input with out_dim %d, %s "
+                             "aggregation and fan-out %d" % (c.in_self, c.out_dim, c.agg_type, max(fanouts)))
+        if rt.world > 1:
+            raise ValueError("learn_input_embedding trains on one GPU only (world = %d)" % rt.world)
+
+    def _make_input_embedding(self, lr: float) -> InputEmbedding:
+        """E ~ truncated normal (+-2 sigma, sigma = 1 / sqrt(d)) from the trainer's seed with its own salt, its bf16 image,
+        Adam moments, gradient table and touched-row bitmap, and the scatter's arguments for layer 1's segments."""
+        from .. import config as _config
+        from ..parallel.runtime import make_table_desc
+        from types import SimpleNamespace
+        rt, n, dev = self.rt, self.nodes.n_local, self.rt.device
+        ly = self.layers[0]
+        c = ly.conv
+        d = c.in_self
+        dp = (d + 7) // 8 * 8
+        g = torch.Generator(device=dev).manual_seed((self.rng.seed * 0x9E3779B1 + self.EMBED_SALT) % 2 ** 63)
+        sigma = d ** -0.5
+        master = torch.zeros(n, dp, dtype=torch.float32, device=dev)
+        torch.nn.init.trunc_normal_(master[:, :d], std=sigma, a=-2 * sigma, b=2 * sigma, generator=g)
+        stride = dp                                                 # 16-byte bf16 rows, line-aligned when wide (set_float)
+        align = int(getattr(_config.get(), "feature_row_align", 128))
+        if align > 16 and d * 2 > align // 2:
+            stride = (d * 2 + align - 1) // align * align // 2
+        table = rt.symm_empty((n, stride), torch.bfloat16)
+        table.local.zero_()
+        table.local[:, :dp] = master.to(torch.bfloat16)
+        desc = make_table_desc(rt.world, d, stride, torch.bfloat16, table.nrows, table.ptrs)
+        k = self.fanouts[:ly.nseg]
+        agg = c.agg_type
+        sscale = [1.0 / (x + 1) if agg == "gcn" else 1.0 for x in k]
+        nscale = [1.0 / x if agg == "mean" else 1.0 / (x + 1) if agg == "gcn" else 1.0 for x in k]
+        scatter = dict(seg_row0=ly.offs[:-1], seg_k=k, self_scale=sscale, nbr_scale=nscale,
+                       nbr_col0=sage_ops.padded_dims(d, d, agg)[0], amax=ly.amax)
+        return InputEmbedding(d=d, table=table, desc=desc,
+                              view=SimpleNamespace(rt=rt, feats=table, feat_desc=desc, float_dim=d),
+                              master=master, m=torch.zeros_like(master), v=torch.zeros_like(master),
+                              grad=torch.zeros_like(master), bits=torch.zeros((n + 31) // 32, dtype=torch.int32, device=dev),
+                              lr=lr, scatter=scatter)
+
+    def input_embedding(self) -> torch.Tensor:
+        """The fp32 master copy of the learned input table E, ``[n_local, d]``, row r = the node with vid
+        ``r * world + rank`` (``utils.checkpoint.save_embeddings`` exports it)."""
+        if self.emb is None:
+            raise ValueError("this trainer was built without learn_input_embedding")
+        return self.emb.master[:, :self.emb.d]
+
+    def _input_desc(self) -> torch.Tensor:
+        """descriptor of the table layer 1 reads: the learned input table, or the node table's float attributes"""
+        return self.nodes.feat_desc if self.emb is None else self.emb.desc
 
     # ------------------------------------------------------------------ GSL front end
     @classmethod
@@ -395,8 +495,8 @@ class FastSageTrainer:
         # ---- forward: ONE persistent launch per layer covering all of its hop-pair segments; the top layer's
         # launch also computes the loss, dlogits and the bias gradient in its epilogue (fused CE)
         for ly in self.layers:
-            if ly.below is None:    # self / neighbour rows: ids of hops i / i + 1 in the feature table
-                d, self_ids, nbr_ids = self.nodes.feat_desc, hops[:ly.nseg], hops[1:ly.nseg + 1]
+            if ly.below is None:    # self / neighbour rows: ids of hops i / i + 1 in the feature (or learned input) table
+                d, self_ids, nbr_ids = self._input_desc(), hops[:ly.nseg], hops[1:ly.nseg + 1]
             else:                   # ... the contiguous row ranges of segments i / i + 1 of the layer below
                 d, self_ids, nbr_ids = ly.below, [None] * ly.nseg, [None] * ly.nseg
             ce = [self.nodes.labels.local, seeds, self.loss, ly.dZ, ly.db] if ly.fuse_ce else []
@@ -427,6 +527,12 @@ class FastSageTrainer:
             if ly.dA is not None:
                 # dA_l [rows, K_total] = dZ_l [rows, n_split * n_img] . W_l
                 C.sage_bwd_da(ly.dZp, ly.img, ly.N, ly.ns, ly.dA, ly.da_alpha)
+        e = self.emb
+        if e is not None:
+            # dA_1 -> the gradient rows of the hop ids layer 1 read (+ their bits in the touched-row bitmap)
+            ly = self.layers[0]
+            C.embed_grad_scatter(ly.dA, self_ids=hops[:ly.nseg], nbr_ids=hops[1:ly.nseg + 1], grad=e.grad, bits=e.bits,
+                                 **e.scatter)
         # ---- join, gradient all-reduce + fused optimiser (Adam + zero grads + next step's weight images)
         main.wait_stream(sA)
         if pipe is not None:
@@ -437,6 +543,12 @@ class FastSageTrainer:
         if self._skip_opt:
             ar(self.flat_g, average=True)
             return
+        if e is not None:
+            # lazy Adam of the touched rows of E beside the dense optimiser, at the step count it uses (advanced above)
+            sA.wait_stream(main)
+            with torch.cuda.stream(sA):
+                C.embed_lazy_adam(e.master, e.m, e.v, e.grad, e.table.local, e.bits, o.step_t, e.lr, o.betas[0],
+                                  o.betas[1], o.eps)
         if ar.backend == "peer":
             # ONE kernel: stage grads (scaled, optionally bf16) -> cross-GPU flag barrier -> pull + reduce every peer's
             # slice in registers -> Adam -> zero grads -> next step's weight images (K8 fused with cast/scale + optimiser)
@@ -447,6 +559,8 @@ class FastSageTrainer:
             ar(self.flat_g, average=True)
             C.adam_pack(self.flat_p, self.g_store, o.m, o.v, o.step_t, o.lr, o.betas[0], o.betas[1], o.eps, o.wd,
                         self.loss_out, self._mats, None, None, None, 1.0, False, self._drop_ctr)
+        if e is not None:
+            main.wait_stream(sA)                        # E is updated before the next step's layer-1 forward reads it
 
     def repack(self):
         """Rebuild the bf16 weight images from the fp32 master weights (after init / load_state_dict / any
@@ -564,7 +678,7 @@ class FastSageTrainer:
     def predict(self, seeds: torch.Tensor) -> torch.Tensor:
         self.model.eval()
         hops = self.sample(seeds)
-        out = self.model.forward_store(self.nodes, hops, self.fanouts)
+        out = self.model.forward_store(self.nodes if self.emb is None else self.emb.view, hops, self.fanouts)
         self.model.train()
         return out
 
@@ -596,7 +710,7 @@ class FastSageTrainer:
             self._inf = (plan, self.nodes.idmap.local_vids(), tabs)
         plan, vids, tabs = self._inf
         rt.barrier()                                                # peers are done reading the previous call's tables
-        desc = self.nodes.feat_desc
+        desc = self._input_desc()
         for l, ly in enumerate(self.layers):
             c = ly.conv
             if ly.last:                                             # image i writes columns [i n_out, i n_out + n_out)
@@ -619,10 +733,15 @@ class FastSageTrainer:
         return float((pred == self.nodes.labels.local[rows]).float().mean())
 
     def state_dict(self):
-        return {"model": self.flat_p.clone(), "opt": self.opt.state_dict(), "rng": self.rng.state_dict(),
-                "steps": self._steps, "dropout_state": self.drop_state.cpu()}
+        sd = {"model": self.flat_p.clone(), "opt": self.opt.state_dict(), "rng": self.rng.state_dict(),
+              "steps": self._steps, "dropout_state": self.drop_state.cpu()}
+        if self.emb is not None:
+            sd["input_embedding"] = {"master": self.emb.master.clone(), "m": self.emb.m.clone(), "v": self.emb.v.clone()}
+        return sd
 
     def load_state_dict(self, sd):
+        if self.emb is not None and "input_embedding" not in sd:
+            raise ValueError("the checkpoint has no learned input embedding, which this trainer trains")
         self.flat_p.copy_(sd["model"])
         self.repack()
         self.opt.load_state_dict(sd["opt"])
@@ -630,3 +749,7 @@ class FastSageTrainer:
         self._steps = int(sd["steps"])
         if "dropout_state" in sd:       # (checkpoints written before dropout training keep this trainer's own state)
             self.drop_state.copy_(sd["dropout_state"])
+        if self.emb is not None:
+            e, s = self.emb, sd["input_embedding"]
+            e.master.copy_(s["master"]); e.m.copy_(s["m"]); e.v.copy_(s["v"])
+            e.table.local[:, :e.master.size(1)] = e.master.to(torch.bfloat16)
