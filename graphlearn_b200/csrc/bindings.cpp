@@ -45,7 +45,8 @@ void sage_fused_csr(const at::Tensor&, const at::Tensor&, const at::Tensor&, con
 int sm_count();
 void sage_set_debug_trace(const c10::optional<at::Tensor>&);
 // sage_bwd.cu
-void sage_bwd_da(const at::Tensor&, const at::Tensor&, int64_t, int64_t, const at::Tensor&, double);
+void sage_bwd_da(const at::Tensor&, const at::Tensor&, int64_t, int64_t, const at::Tensor&, double,
+                 const std::vector<std::pair<int64_t, int64_t>>&);
 void sage_bwd_dw(const c10::optional<at::Tensor>&, const c10::optional<at::Tensor>&, const std::vector<int64_t>&,
                  const std::vector<int64_t>&, const std::vector<c10::optional<at::Tensor>>&,
                  const std::vector<c10::optional<at::Tensor>>&, const std::vector<int64_t>&, const std::vector<double>&, int64_t,
@@ -200,9 +201,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("self_src"), py::arg("nbr_src"), py::arg("seg_k"), py::arg("seg_scale"), py::arg("nbr_col0"), py::arg("dz_out"),
         py::arg("a"), py::arg("dw"), py::arg("dbias"), py::arg("n_out"), py::arg("seg_self_scale") = std::vector<double>(),
         py::arg("amax_src") = std::vector<c10::optional<at::Tensor>>());
-  // (alpha: scale of the fp32 accumulators before the bf16 store, 1 / (1 - p) below a dropout layer)
+  // (alpha: scale of the fp32 accumulators before the bf16 store, 1 / (1 - p) below a dropout layer; kb_ranges: at most
+  // two [lo, hi) ranges of 64-column blocks of da to compute, empty = all)
   m.def("sage_bwd_da", &glb::sage_bwd_da, py::arg("dz"), py::arg("w_img"), py::arg("N"), py::arg("n_imgs"), py::arg("da"),
-        py::arg("alpha") = 1.0);
+        py::arg("alpha") = 1.0, py::arg("kb_ranges") = std::vector<std::pair<int64_t, int64_t>>());
   m.def("embed_grad_scatter", &glb::embed_grad_scatter, py::arg("da"), py::arg("seg_row0"), py::arg("self_ids"),
         py::arg("nbr_ids"), py::arg("seg_k"), py::arg("self_scale"), py::arg("nbr_scale"), py::arg("nbr_col0"), py::arg("amax"),
         py::arg("grad"), py::arg("bits"));

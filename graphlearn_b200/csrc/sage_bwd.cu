@@ -410,18 +410,20 @@ void sage_bwd_dw(const c10::optional<at::Tensor>& dz, const c10::optional<at::Te
 // reduction steps in flight, the accumulators of all 64 output columns in registers.  The B fragments come from the block by
 // ldmatrix.trans: each 8x8 matrix is 8 consecutive block rows at one 16-byte chunk, which the swizzle spreads over 8
 // different bank groups (N is a multiple of 8, so the images' swizzle atoms line up in the concatenated block).
-// grid = (K_total / 64, min(ceil(rows / 64), kDaCtasPerSm * SMs / (K_total / 64))) x 128 threads: when there are more row
-// blocks than that, a CTA keeps its W block and walks row blocks y, y + gridDim.y, ... (a wide layer's block is up to
-// 64 KB, and re-staging it for every 64 rows would cost more L2 traffic than the dZ rows themselves).
+// grid = (B, min(ceil(rows / 64), kDaCtasPerSm * SMs / B)) x 128 threads, B = the 64-column blocks computed (all K_total / 64
+// of them, or those of at most two windows [lo0, lo0 + n0) and [lo1, ...)): when there are more row blocks than that, a CTA
+// keeps its W block and walks row blocks y, y + gridDim.y, ... (a wide layer's block is up to 64 KB, and re-staging it for
+// every 64 rows would cost more L2 traffic than the dZ rows themselves).
 constexpr int kDaThreads = 128;
 constexpr int kDaMaxR = 512;
 constexpr int kDaCtasPerSm = 4;
 
 __global__ void __launch_bounds__(kDaThreads) sage_bwd_da_kernel(const __nv_bfloat16* __restrict__ dz, int ld_dz, int rows,
-                                                                 const uint8_t* __restrict__ w_img, int N, int n_imgs,
+                                                                 const uint8_t* __restrict__ w_img, int N, int n_imgs, int nkb,
+                                                                 int lo0, int n0, int lo1,
                                                                  __nv_bfloat16* __restrict__ da, int ld_da, float alpha) {
   extern __shared__ __align__(128) uint8_t sW[];
-  const int kb = blockIdx.x, nkb = gridDim.x;
+  const int kb = (int)blockIdx.x < n0 ? lo0 + (int)blockIdx.x : lo1 + ((int)blockIdx.x - n0);
   const int R = n_imgs * N;
   const uint32_t w_base = gmma::smem_u32(sW);
   // the W block arrives by cp.async, overlapped with the first dZ loads
@@ -503,7 +505,10 @@ __global__ void __launch_bounds__(kDaThreads) sage_bwd_da_kernel(const __nv_bflo
 // columns each ([n_imgs][K_total / 64][N][64], zero rows beyond the real outputs), R = n_imgs * N; dZ columns [n_out, R)
 // must be zero or finite.  alpha scales the fp32 accumulators before the bf16 store (alpha = 1 is exact): 1 / (1 - p)
 // when the layer's input was dropped out with rate p, which leaves dZ itself unscaled for the weight gradient.
-void sage_bwd_da(const at::Tensor& dz, const at::Tensor& w_img, int64_t N, int64_t n_imgs, const at::Tensor& da, double alpha) {
+// kb_ranges: empty = every 64-column block of dA; else at most two disjoint half-open ranges [lo, hi) of blocks, and only
+// their columns are written (the learned input embedding's layer 1 needs the gradient of E's columns, not the features').
+void sage_bwd_da(const at::Tensor& dz, const at::Tensor& w_img, int64_t N, int64_t n_imgs, const at::Tensor& da, double alpha,
+                 const std::vector<std::pair<int64_t, int64_t>>& kb_ranges) {
   const int64_t R = n_imgs * N;
   TORCH_CHECK(N % 8 == 0 && N >= 8 && n_imgs >= 1 && R % 32 == 0 && R <= kDaMaxR,
               "sage_bwd_da needs n_imgs images of N output columns (N a multiple of 8), n_imgs * N a multiple of 32 in [32, ",
@@ -527,10 +532,20 @@ void sage_bwd_da(const at::Tensor& dz, const at::Tensor& w_img, int64_t N, int64
     attr_done = true;
   }
   const int64_t nkb = k_total / 64, row_blocks = (rows + 63) / 64;
-  const dim3 grid((unsigned)nkb, (unsigned)std::min<int64_t>(row_blocks, std::max<int64_t>(1, kDaCtasPerSm * sm_count() / nkb)));
+  TORCH_CHECK(kb_ranges.size() <= 2, "sage_bwd_da takes at most two column-block ranges");
+  for (const auto& r : kb_ranges)
+    TORCH_CHECK(0 <= r.first && r.first < r.second && r.second <= nkb, "sage_bwd_da: column-block range [", r.first, ", ",
+                r.second, ") is empty or outside the ", nkb, " blocks of da");
+  TORCH_CHECK(kb_ranges.size() < 2 || kb_ranges[0].second <= kb_ranges[1].first || kb_ranges[1].second <= kb_ranges[0].first,
+              "sage_bwd_da: the column-block ranges overlap");
+  const int64_t lo0 = kb_ranges.empty() ? 0 : kb_ranges[0].first;
+  const int64_t n0 = kb_ranges.empty() ? nkb : kb_ranges[0].second - lo0;
+  const int64_t lo1 = kb_ranges.size() < 2 ? 0 : kb_ranges[1].first;
+  const int64_t blocks = n0 + (kb_ranges.size() < 2 ? 0 : kb_ranges[1].second - lo1);
+  const dim3 grid((unsigned)blocks, (unsigned)std::min<int64_t>(row_blocks, std::max<int64_t>(1, kDaCtasPerSm * sm_count() / blocks)));
   sage_bwd_da_kernel<<<grid, kDaThreads, (size_t)R * 128, at::cuda::getCurrentCUDAStream()>>>(
       bf16_ptr(dz), (int)dz.stride(0), (int)rows, reinterpret_cast<const uint8_t*>(w_img.data_ptr()), (int)N, (int)n_imgs,
-      reinterpret_cast<__nv_bfloat16*>(da.data_ptr()), (int)da.stride(0), (float)alpha);
+      (int)nkb, (int)lo0, (int)n0, (int)lo1, reinterpret_cast<__nv_bfloat16*>(da.data_ptr()), (int)da.stride(0), (float)alpha);
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
 

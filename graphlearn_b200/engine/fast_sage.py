@@ -26,13 +26,17 @@ seed is the sampler's per-rank seed with its own salt; the counter is advanced b
 launch of the step.  No mask is stored: H_l > 0 exactly where m * relu'(Z_l) = 1, so the dW kernel's relu'(H_l) test
 applies the mask and ``sage_bwd_da`` of layer l + 1 applies the 1 / (1 - p).
 
-Learned input embedding (``learn_input_embedding=True``, for node tables without float attributes): layer 1 reads a
-trainable table E ``[n_local, d]`` (d = the first layer's input width) through its bf16 image, as it reads a feature
-table otherwise.  The backward adds three launches: dW_1 also stores dZ_1 (and a max layer 1's forward its argmax bytes),
-dA_1 = dZ_1 W_1 runs on ``sage_bwd_da``, and ``embed_grad_scatter`` adds the self / neighbour halves of dA_1 (scaled like
-the layer's aggregator) into an fp32 gradient table and marks the rows read in a bitmap.  ``embed_lazy_adam`` then updates
-the touched rows only (``torch.optim.SparseAdam``'s semantics at the dense Adam's step count), rewrites their bf16 image
-rows and clears their gradient rows and bits, on a branch beside ``adam_pack``.
+Learned input embedding (``learn_input_embedding=True``): layer 1 reads a trainable table E ``[n_local, d]`` through a
+bf16 image, as it reads a feature table otherwise.  Without float attributes, d is the first layer's input width.  With
+f = ``nodes.float_dim`` > 0 float attributes, layer 1's input row is ``[E_r || x_r]``, d = in_dim - f: image columns
+[0, d) hold E and [d, d + f) the attributes rounded to bf16, and the columns of each half of W_1 follow that order.  The
+attribute columns are a snapshot taken at construction (training never writes them; a later ``set_float`` on the node
+table is not seen).  The backward adds three launches: dW_1 also stores dZ_1 (and a max layer 1's forward its argmax
+bytes), dA_1 = dZ_1 W_1 runs on ``sage_bwd_da`` (with attributes: only over the 64-column blocks that hold E's columns),
+and ``embed_grad_scatter`` adds the self / neighbour halves of dA_1 (scaled like the layer's aggregator) into an fp32
+gradient table and marks the rows read in a bitmap.  ``embed_lazy_adam`` then updates the touched rows only
+(``torch.optim.SparseAdam``'s semantics at the dense Adam's step count), rewrites their E columns of the image and
+clears their gradient rows and bits, on a branch beside ``adam_pack``.
 
 9 launches of this repo's kernels (0 library kernels) for the 2-layer flagship instead of ~60 on the autograd path
 (12 with the learned input embedding).
@@ -92,6 +96,9 @@ class SageLayer:
     # p > 0; (None, 0.0, 0, []) otherwise)
     drop: tuple
     da_alpha: float                 # scale of dA: 1 / (1 - p) when the layer's input H_{l-1} is dropped out, else 1
+    # sage_bwd_da's kb_ranges: the 64-column blocks of dA it computes, () = all (layer 1 with a learned input embedding
+    # next to float attributes: only E's blocks of each half, nobody reads the attributes' gradient)
+    da_blocks: tuple = ()
     # max aggregation, l >= 2: uint8 [rows, in_nbr padded to 16], row m of segment i = for each neighbour-half column the
     # first of the k neighbours holding its max, written by the forward (`amax` per-segment views) for the layer below's
     # gradient routing; layer 1 has them only when it reads the learned input table (a feature table has no gradient)
@@ -105,10 +112,13 @@ class SageLayer:
 @dataclass
 class InputEmbedding:
     """The learned layer-1 input table E ``[n_local, d]`` of a trainer built with ``learn_input_embedding=True``: row r
-    is the node with vid ``r * world + rank``.  Layer 1 reads its bf16 image; the fp32 tables (master, Adam moments,
-    gradient) have ``dp = d`` rounded up to 8 columns, whose padding stays zero."""
+    is the node with vid ``r * world + rank``.  Layer 1 reads the bf16 image ``[E || x]`` (x: the node table's f float
+    attributes, f = 0 without them); the fp32 tables (master, Adam moments, gradient) have ``dp = d`` rounded up to 8
+    columns, whose padding stays zero (with attributes d is a multiple of 8, so dp = d)."""
     d: int
-    table: object                   # SymmTensor: bf16 image [n_local, stride], stride by the feature tables' rules
+    f: int
+    table: object                   # SymmTensor: bf16 image [n_local, stride] (E in [0, d), x in [d, d + f)), stride by
+                                    # the feature tables' rules
     desc: torch.Tensor              # its table descriptor (what layer 1 reads where a feature table's is read otherwise)
     view: object                    # NodeTable-like (rt, feats, feat_desc, float_dim) over the image: predict / embed
     master: torch.Tensor            # fp32 [n_local, dp]
@@ -256,10 +266,16 @@ class FastSageTrainer:
     @staticmethod
     def _check_input_embedding(rt: Runtime, nodes: NodeTable, model, fanouts: Sequence[int]):
         c = model.convs[0]
-        if nodes.float_dim > 0:
-            raise ValueError("learn_input_embedding replaces the node table's float attributes as the layer-1 input; this "
-                             "table has %d of them (concatenating attributes with a learned embedding is not supported)"
-                             % nodes.float_dim)
+        f = nodes.float_dim
+        if f > 0 and c.in_self <= f:
+            raise ValueError("learn_input_embedding concatenates a learned embedding with the node table's %d float "
+                             "attributes: the first layer's input width (%d) leaves no columns for it" % (f, c.in_self))
+        if f > 0 and (c.in_self - f) % 8 != 0:
+            raise ValueError("learn_input_embedding next to float attributes needs an embedding width (input width %d - "
+                             "%d attributes = %d) that is a multiple of 8" % (c.in_self, f, c.in_self - f))
+        if f > 0 and nodes.feats.local.dtype not in (torch.float32, torch.bfloat16):
+            raise ValueError("learn_input_embedding reads float attributes from fp32 or bf16 node tables (this one stores "
+                             "block-scaled fp8)")
         if c.in_self != c.in_nbr:
             raise ValueError("learn_input_embedding needs the first layer's self and neighbour input widths to be equal "
                              "(got %d and %d)" % (c.in_self, c.in_nbr))
@@ -271,36 +287,49 @@ class FastSageTrainer:
             raise ValueError("learn_input_embedding trains on one GPU only (world = %d)" % rt.world)
 
     def _make_input_embedding(self, lr: float) -> InputEmbedding:
-        """E ~ truncated normal (+-2 sigma, sigma = 1 / sqrt(d)) from the trainer's seed with its own salt, its bf16 image,
-        Adam moments, gradient table and touched-row bitmap, and the scatter's arguments for layer 1's segments."""
+        """E ~ truncated normal (+-2 sigma, sigma = 1 / sqrt(d)) from the trainer's seed with its own salt, the bf16
+        image [E || x], Adam moments, gradient table and touched-row bitmap, and the scatter's arguments for layer 1's
+        segments."""
         from .. import config as _config
+        from ..ops.gather import gather_rows
         from ..parallel.runtime import make_table_desc
         from types import SimpleNamespace
-        rt, n, dev = self.rt, self.nodes.n_local, self.rt.device
+        rt, nodes, dev = self.rt, self.nodes, self.rt.device
+        n, f = nodes.n_local, nodes.float_dim
         ly = self.layers[0]
         c = ly.conv
-        d = c.in_self
+        width = c.in_self                                           # d + f columns of a layer-1 input row
+        d = width - f
         dp = (d + 7) // 8 * 8
         g = torch.Generator(device=dev).manual_seed((self.rng.seed * 0x9E3779B1 + self.EMBED_SALT) % 2 ** 63)
         sigma = d ** -0.5
         master = torch.zeros(n, dp, dtype=torch.float32, device=dev)
         torch.nn.init.trunc_normal_(master[:, :d], std=sigma, a=-2 * sigma, b=2 * sigma, generator=g)
-        stride = dp                                                 # 16-byte bf16 rows, line-aligned when wide (set_float)
+        stride = (width + 7) // 8 * 8                               # 16-byte bf16 rows, line-aligned when wide (set_float)
         align = int(getattr(_config.get(), "feature_row_align", 128))
-        if align > 16 and d * 2 > align // 2:
-            stride = (d * 2 + align - 1) // align * align // 2
+        if align > 16 and width * 2 > align // 2:
+            stride = (width * 2 + align - 1) // align * align // 2
         table = rt.symm_empty((n, stride), torch.bfloat16)
         table.local.zero_()
         table.local[:, :dp] = master.to(torch.bfloat16)
-        desc = make_table_desc(rt.world, d, stride, torch.bfloat16, table.nrows, table.ptrs)
+        if f > 0:                   # the attributes, rounded to bf16 once (training never writes these columns)
+            table.local[:, d:width] = gather_rows(rt, nodes.feats, nodes.feat_desc, nodes.idmap.local_vids(),
+                                                  f).to(torch.bfloat16)
+        desc = make_table_desc(rt.world, width, stride, torch.bfloat16, table.nrows, table.ptrs)
         k = self.fanouts[:ly.nseg]
         agg = c.agg_type
         sscale = [1.0 / (x + 1) if agg == "gcn" else 1.0 for x in k]
         nscale = [1.0 / x if agg == "mean" else 1.0 / (x + 1) if agg == "gcn" else 1.0 for x in k]
-        scatter = dict(seg_row0=ly.offs[:-1], seg_k=k, self_scale=sscale, nbr_scale=nscale,
-                       nbr_col0=sage_ops.padded_dims(d, d, agg)[0], amax=ly.amax)
-        return InputEmbedding(d=d, table=table, desc=desc,
-                              view=SimpleNamespace(rt=rt, feats=table, feat_desc=desc, float_dim=d),
+        nbr_col0 = sage_ops.padded_dims(width, width, agg)[0]
+        scatter = dict(seg_row0=ly.offs[:-1], seg_k=k, self_scale=sscale, nbr_scale=nscale, nbr_col0=nbr_col0,
+                       amax=ly.amax)
+        if f > 0:
+            # dA_1 over E's 64-column blocks of the self half [0, d) and of the neighbour half [nbr_col0, nbr_col0 + d)
+            # (gcn: one shared half at column 0): the attributes' columns of dA_1 would be most of its bytes, unread
+            nb = (d + 63) // 64
+            ly.da_blocks = ((0, nb),) + (((nbr_col0 // 64, nbr_col0 // 64 + nb),) if nbr_col0 else ())
+        return InputEmbedding(d=d, f=f, table=table, desc=desc,
+                              view=SimpleNamespace(rt=rt, feats=table, feat_desc=desc, float_dim=width),
                               master=master, m=torch.zeros_like(master), v=torch.zeros_like(master),
                               grad=torch.zeros_like(master), bits=torch.zeros((n + 31) // 32, dtype=torch.int32, device=dev),
                               lr=lr, scatter=scatter)
@@ -526,7 +555,7 @@ class FastSageTrainer:
                 C.sage_bwd_dw(None, ly.H, a=ly.A, dw=ly.dW, dbias=ly.db, n_out=ly.conv.out_dim, **ly.bwd)
             if ly.dA is not None:
                 # dA_l [rows, K_total] = dZ_l [rows, n_split * n_img] . W_l
-                C.sage_bwd_da(ly.dZp, ly.img, ly.N, ly.ns, ly.dA, ly.da_alpha)
+                C.sage_bwd_da(ly.dZp, ly.img, ly.N, ly.ns, ly.dA, ly.da_alpha, ly.da_blocks)
         e = self.emb
         if e is not None:
             # dA_1 -> the gradient rows of the hop ids layer 1 read (+ their bits in the touched-row bitmap)
