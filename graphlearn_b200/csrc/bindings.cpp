@@ -50,8 +50,17 @@ void sage_bwd_da(const at::Tensor&, const at::Tensor&, int64_t, int64_t, const a
 void sage_bwd_dw(const c10::optional<at::Tensor>&, const c10::optional<at::Tensor>&, const std::vector<int64_t>&,
                  const std::vector<int64_t>&, const std::vector<c10::optional<at::Tensor>>&,
                  const std::vector<c10::optional<at::Tensor>>&, const std::vector<int64_t>&, const std::vector<double>&, int64_t,
-                 const c10::optional<at::Tensor>&, const at::Tensor&, const at::Tensor&, const c10::optional<at::Tensor>&, int64_t,
-                 const std::vector<double>&, const std::vector<c10::optional<at::Tensor>>&);
+                 const c10::optional<at::Tensor>&, const c10::optional<at::Tensor>&, const c10::optional<at::Tensor>&,
+                 const c10::optional<at::Tensor>&, int64_t, const std::vector<double>&, const std::vector<c10::optional<at::Tensor>>&);
+// sage_bn.cu
+void bn_fwd_stats(const at::Tensor&, int64_t, const std::vector<int64_t>&, const at::Tensor&, const at::Tensor&, const at::Tensor&,
+                  const at::Tensor&, const at::Tensor&, const at::Tensor&, double, double);
+void bn_fwd_apply(const at::Tensor&, int64_t, const std::vector<int64_t>&, const at::Tensor&, const at::Tensor&, const at::Tensor&,
+                  const at::Tensor&, const at::Tensor&, const c10::optional<at::Tensor>&, double, int64_t);
+void bn_bwd_reduce(const at::Tensor&, const at::Tensor&, int64_t, const std::vector<int64_t>&, const at::Tensor&, const at::Tensor&,
+                   const at::Tensor&, const at::Tensor&, const at::Tensor&, const at::Tensor&);
+void bn_bwd_apply(const at::Tensor&, const at::Tensor&, int64_t, const std::vector<int64_t>&, const at::Tensor&, const at::Tensor&,
+                  const at::Tensor&, const at::Tensor&, const at::Tensor&);
 // sage_embed.cu
 void embed_grad_scatter(const at::Tensor&, const std::vector<int64_t>&, const std::vector<at::Tensor>&, const std::vector<at::Tensor>&,
                         const std::vector<int64_t>&, const std::vector<double>&, const std::vector<double>&, int64_t,
@@ -205,6 +214,17 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   // two [lo, hi) ranges of 64-column blocks of da to compute, empty = all)
   m.def("sage_bwd_da", &glb::sage_bwd_da, py::arg("dz"), py::arg("w_img"), py::arg("N"), py::arg("n_imgs"), py::arg("da"),
         py::arg("alpha") = 1.0, py::arg("kb_ranges") = std::vector<std::pair<int64_t, int64_t>>());
+  // batch norm of a hidden layer's segments (offs: the nseg + 1 row offsets), see sage_bn.cu
+  m.def("bn_fwd_stats", &glb::bn_fwd_stats, py::arg("z"), py::arg("C"), py::arg("offs"), py::arg("ticket"), py::arg("mean"),
+        py::arg("rstd"), py::arg("running_mean"), py::arg("running_var"), py::arg("num_batches_tracked"), py::arg("eps"),
+        py::arg("momentum"));
+  m.def("bn_fwd_apply", &glb::bn_fwd_apply, py::arg("z"), py::arg("C"), py::arg("offs"), py::arg("mean"), py::arg("rstd"),
+        py::arg("gamma"), py::arg("beta"), py::arg("h"), py::arg("drop_state") = py::none(), py::arg("drop_p") = 0.0,
+        py::arg("drop_layer") = 0);
+  m.def("bn_bwd_reduce", &glb::bn_bwd_reduce, py::arg("dy"), py::arg("z"), py::arg("C"), py::arg("offs"), py::arg("ticket"),
+        py::arg("mean"), py::arg("rstd"), py::arg("gsum"), py::arg("dgamma"), py::arg("dbeta"));
+  m.def("bn_bwd_apply", &glb::bn_bwd_apply, py::arg("dy"), py::arg("z"), py::arg("C"), py::arg("offs"), py::arg("mean"),
+        py::arg("rstd"), py::arg("gamma"), py::arg("gsum"), py::arg("dz"));
   m.def("embed_grad_scatter", &glb::embed_grad_scatter, py::arg("da"), py::arg("seg_row0"), py::arg("self_ids"),
         py::arg("nbr_ids"), py::arg("seg_k"), py::arg("self_scale"), py::arg("nbr_scale"), py::arg("nbr_col0"), py::arg("amax"),
         py::arg("grad"), py::arg("bits"));

@@ -20,6 +20,10 @@
 // neighbour part only to the child j = (r - row0) % k that held the maximum:
 //     dZ_l[r, c] = relu'(H_l[r, c]) * ( sscale * self[c]  +  scale * [amax[parent][c] == j] * nbr[c] )
 //
+// sage_bwd_dz_kernel is the dZ-only mode of the same body (DW = false, no `a` / `dw`): the producers compute and store dZ
+// to dz_out and nothing else runs (no A loads, no MMAs) - the batch-normalised layer's dY, whose dW follows from the
+// normalised gradient on the dense-dZ path.
+//
 // warps 0..15 : producers (loads -> ReLU-grad math -> swizzled st.shared) and, as four warpgroups, the MMA issuers:
 //               warpgroup g owns the [64 x 64] quadrant (rows 64 (g & 1), columns 64 (g >> 1)) of the CTA's dW block
 //               and issues its MMAs of a stage once all 16 warps have filled it (3-stage mbarrier ring, operands of
@@ -86,8 +90,8 @@ __device__ __forceinline__ uint32_t mn_off(int r, int c) {
   return (uint32_t)(c >> 3) * 8192u + (uint32_t)(r >> 3) * 1024u + (uint32_t)(r & 7) * 128u + (uint32_t)(((c & 7) ^ (r & 7)) << 4);
 }
 
-template <bool ROUTE>
-__global__ void __launch_bounds__(kDwThreads, 1) sage_bwd_dw_kernel(const __grid_constant__ DwParams p) {
+template <bool ROUTE, bool DW>
+__device__ __forceinline__ void sage_bwd_dw_body(const DwParams& p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (gmma::smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* stages = smem;
@@ -139,10 +143,12 @@ __global__ void __launch_bounds__(kDwThreads, 1) sage_bwd_dw_kernel(const __grid
     struct StageRegs { uint4 bv[2], hv[2], sv[2], nv[2]; float nscale[2]; uint2 am[2]; uint32_t j[2]; float sscale[2]; };
     auto issue = [&](int st, StageRegs& g) {
       const int rbase = r_begin + st * kDwRows;
+      if constexpr (DW) {
 #pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        const int r = rbase + br + 32 * i;
-        g.bv[i] = (r < r_end && bcol_ok) ? ldg16(p.a + (size_t)r * p.ld_a + bcol) : zero4;
+        for (int i = 0; i < 2; ++i) {
+          const int r = rbase + br + 32 * i;
+          g.bv[i] = (r < r_end && bcol_ok) ? ldg16(p.a + (size_t)r * p.ld_a + bcol) : zero4;
+        }
       }
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
@@ -210,6 +216,7 @@ __global__ void __launch_bounds__(kDwThreads, 1) sage_bwd_dw_kernel(const __grid
         const int r = rbase + zr + 32 * i;
         if (want_out && r < r_end && zcol < p.ld_dz_out) *reinterpret_cast<uint4*>(p.dz_out + (size_t)r * p.ld_dz_out + zcol) = zv[i];
       }
+      if constexpr (!DW) return;
       gmma::mbar_wait(bar_empty + s, (uint32_t)(((st / kDwStages) & 1) ^ 1));
       uint8_t* zs = stages + (size_t)s * kDwStageBytes;
       uint8_t* bs = zs + kDwZBytes;
@@ -251,8 +258,10 @@ __global__ void __launch_bounds__(kDwThreads, 1) sage_bwd_dw_kernel(const __grid
     // bias gradient = column sums of the computed dZ (only the n-block-0 CTAs of an m-block contribute): the two
     // rows of a warp are folded with a shuffle, every warp parks its 128 sums in the (now idle) stage memory and
     // 128 threads add the 16 rows up - no shared-memory atomics (they were 32-way same-address conflicts)
-    gmma::wgmma_wait<0>();
-    gmma::fence_regs(acc);
+    if constexpr (DW) {
+      gmma::wgmma_wait<0>();
+      gmma::fence_regs(acc);
+    }
     const bool do_bias = p.dbias && !p.dz && nb == 0 && n_steps > 0;
     if (do_bias) {
 #pragma unroll
@@ -274,7 +283,7 @@ __global__ void __launch_bounds__(kDwThreads, 1) sage_bwd_dw_kernel(const __grid
     atomicAdd(p.dbias + mb * 128 + tid, v);
   }
   // ------------------------------------------------------------------ epilogue: registers -> red.global.add into dW
-  if (n_steps > 0 && wg_active) {
+  if (DW && n_steps > 0 && wg_active) {
     const int r0 = mh * 64 + wq * 16 + (lane >> 2);
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
@@ -290,20 +299,32 @@ __global__ void __launch_bounds__(kDwThreads, 1) sage_bwd_dw_kernel(const __grid
   }
 }
 
-static const __nv_bfloat16* bf16_ptr(const at::Tensor& t) { return reinterpret_cast<const __nv_bfloat16*>(t.data_ptr()); }
+template <bool ROUTE>
+__global__ void __launch_bounds__(kDwThreads, 1) sage_bwd_dw_kernel(const __grid_constant__ DwParams p) {
+  sage_bwd_dw_body<ROUTE, true>(p);
+}
 
 template <bool ROUTE>
+__global__ void __launch_bounds__(kDwThreads, 1) sage_bwd_dz_kernel(const __grid_constant__ DwParams p) {
+  sage_bwd_dw_body<ROUTE, false>(p);
+}
+
+static const __nv_bfloat16* bf16_ptr(const at::Tensor& t) { return reinterpret_cast<const __nv_bfloat16*>(t.data_ptr()); }
+
+template <bool ROUTE, bool DW>
 static void launch_dw(const DwParams& p, int grid, size_t smem) {
   static bool attr_done = false;
+  auto* kernel = DW ? sage_bwd_dw_kernel<ROUTE> : sage_bwd_dz_kernel<ROUTE>;
   if (!attr_done) {
-    C10_CUDA_CHECK(cudaFuncSetAttribute(sage_bwd_dw_kernel<ROUTE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    C10_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr_done = true;
   }
-  sage_bwd_dw_kernel<ROUTE><<<grid, kDwThreads, smem, at::cuda::getCurrentCUDAStream()>>>(p);
+  kernel<<<grid, kDwThreads, smem, at::cuda::getCurrentCUDAStream()>>>(p);
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
 
 // dW (+)= dZ^T A with dZ either dense (`dz`) or computed from (h, segments of dA_next).
+//   a = dw = None: only dZ, computed from (h, segments of dA_next), is written to dz_out ([rows, >= n_out]), nothing else
 //   segs: rows [row0, row1) of the layer; self_src[i] / nbr_src[i] are views into dA_next (or None)
 //   seg_self_scale: [] (all 1) or the self part's scale per segment (gcn above: 1 / (k + 1))
 //   amax_src: [] or per segment None / the uint8 argmax rows of the parents (max above; aligned with nbr_src[i], >= n_out
@@ -312,21 +333,34 @@ void sage_bwd_dw(const c10::optional<at::Tensor>& dz, const c10::optional<at::Te
                  const std::vector<int64_t>& seg_row0, const std::vector<int64_t>& seg_row1,
                  const std::vector<c10::optional<at::Tensor>>& self_src, const std::vector<c10::optional<at::Tensor>>& nbr_src,
                  const std::vector<int64_t>& seg_k, const std::vector<double>& seg_scale, int64_t nbr_col0,
-                 const c10::optional<at::Tensor>& dz_out, const at::Tensor& a, const at::Tensor& dw,
-                 const c10::optional<at::Tensor>& dbias, int64_t n_out, const std::vector<double>& seg_self_scale,
-                 const std::vector<c10::optional<at::Tensor>>& amax_src) {
-  TORCH_CHECK(a.is_cuda() && a.scalar_type() == at::kBFloat16 && a.dim() == 2 && a.stride(1) == 1 && a.stride(0) % 8 == 0);
-  TORCH_CHECK(dw.is_cuda() && dw.scalar_type() == at::kFloat && dw.dim() == 2 && dw.stride(1) == 1 && dw.size(0) >= n_out &&
-              dw.size(1) == a.size(1) && dw.stride(0) % 4 == 0 && (reinterpret_cast<uintptr_t>(dw.data_ptr()) & 15) == 0,
-              "dw must be fp32 [n_out, K_total], 16-byte aligned rows");
-  c10::cuda::CUDAGuard guard(a.device());
+                 const c10::optional<at::Tensor>& dz_out, const c10::optional<at::Tensor>& a_opt,
+                 const c10::optional<at::Tensor>& dw_opt, const c10::optional<at::Tensor>& dbias, int64_t n_out,
+                 const std::vector<double>& seg_self_scale, const std::vector<c10::optional<at::Tensor>>& amax_src) {
+  const bool want_dw = a_opt.has_value() && a_opt->defined();
+  TORCH_CHECK(want_dw == (dw_opt.has_value() && dw_opt->defined()), "sage_bwd_dw: pass both a and dw, or neither");
   DwParams p;
   std::memset(&p, 0, sizeof(p));
   bool route = false;
-  p.rows = (int)a.size(0); p.n_cols = (int)a.size(1); p.n_out = (int)n_out;
-  TORCH_CHECK(p.n_cols % 16 == 0, "K_total must be a multiple of 16");
-  p.a = bf16_ptr(a); p.ld_a = (int)a.stride(0);
-  p.dw = dw.data_ptr<float>(); p.ld_dw = (int)dw.stride(0);
+  p.n_out = (int)n_out;
+  if (want_dw) {
+    const at::Tensor& a = *a_opt;
+    const at::Tensor& dw = *dw_opt;
+    TORCH_CHECK(a.is_cuda() && a.scalar_type() == at::kBFloat16 && a.dim() == 2 && a.stride(1) == 1 && a.stride(0) % 8 == 0);
+    TORCH_CHECK(dw.is_cuda() && dw.scalar_type() == at::kFloat && dw.dim() == 2 && dw.stride(1) == 1 && dw.size(0) >= n_out &&
+                dw.size(1) == a.size(1) && dw.stride(0) % 4 == 0 && (reinterpret_cast<uintptr_t>(dw.data_ptr()) & 15) == 0,
+                "dw must be fp32 [n_out, K_total], 16-byte aligned rows");
+    p.rows = (int)a.size(0); p.n_cols = (int)a.size(1);
+    TORCH_CHECK(p.n_cols % 16 == 0, "K_total must be a multiple of 16");
+    p.a = bf16_ptr(a); p.ld_a = (int)a.stride(0);
+    p.dw = dw.data_ptr<float>(); p.ld_dw = (int)dw.stride(0);
+  } else {
+    TORCH_CHECK(dz_out.has_value() && dz_out->defined() && !(dz.has_value() && dz->defined()) && !(dbias.has_value() && dbias->defined()),
+                "sage_bwd_dw without a / dw computes the routed dZ into dz_out only (no dz, no dbias)");
+    p.rows = (int)dz_out->size(0);
+  }
+  const at::Tensor& dev_t = want_dw ? *a_opt : *dz_out;
+  TORCH_CHECK(dev_t.is_cuda());
+  c10::cuda::CUDAGuard guard(dev_t.device());
   if (dbias.has_value() && dbias->defined()) {
     TORCH_CHECK(dbias->scalar_type() == at::kFloat && dbias->numel() >= n_out);
     p.dbias = dbias->data_ptr<float>();
@@ -345,6 +379,7 @@ void sage_bwd_dw(const c10::optional<at::Tensor>& dz, const c10::optional<at::Te
     p.nbr_col0 = (int)nbr_col0;
     TORCH_CHECK(n_out % 8 == 0 && nbr_col0 % 8 == 0, "hidden width must be a multiple of 8");
     p.dz_cols = (int)n_out;
+    TORCH_CHECK(want_dw || seg_row1[nseg - 1] <= p.rows, "sage_bwd_dw: the segments run past dz_out's rows");
     for (int i = 0; i < nseg; ++i) {
       BwdSeg& g = p.seg[i];
       g.row0 = (int)seg_row0[i]; g.row1 = (int)seg_row1[i]; g.k = (int)std::max<int64_t>(seg_k[i], 1); g.scale = (float)seg_scale[i];
@@ -388,7 +423,7 @@ void sage_bwd_dw(const c10::optional<at::Tensor>& dz, const c10::optional<at::Te
   }
   if (p.rows == 0) return;
   p.m_blocks = (p.n_out + 127) / 128;
-  p.n_blocks = (p.n_cols + kDwCols - 1) / kDwCols;
+  p.n_blocks = want_dw ? (p.n_cols + kDwCols - 1) / kDwCols : 1;
   const int blocks = p.m_blocks * p.n_blocks;
   const int sms = sm_count();
   const int max_splits = std::max(1, sms / blocks);
@@ -398,8 +433,14 @@ void sage_bwd_dw(const c10::optional<at::Tensor>& dz, const c10::optional<at::Te
   const int splits = (p.rows + rps - 1) / rps;
   p.lbo = 8192; p.sbo = 1024; p.kadv = 2048;
   const size_t smem = 1024 + (size_t)kDwStages * kDwStageBytes + 512 + 2 * kDwStages * 8;
-  if (route) launch_dw<true>(p, blocks * splits, smem);
-  else launch_dw<false>(p, blocks * splits, smem);
+  if (!want_dw) {
+    if (route) launch_dw<true, false>(p, blocks * splits, smem);
+    else launch_dw<false, false>(p, blocks * splits, smem);
+  } else if (route) {
+    launch_dw<true, true>(p, blocks * splits, smem);
+  } else {
+    launch_dw<false, true>(p, blocks * splits, smem);
+  }
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -41,6 +41,7 @@
 #include "host_utils.h"
 #include "gmma.cuh"
 #include "gather_common.cuh"
+#include "dropout.cuh"
 
 namespace glb {
 
@@ -201,16 +202,11 @@ __device__ __forceinline__ void store_pair(const SageParams& p, const SageSeg& s
   }
 }
 
-// Dropout mask bits of row `row` of a layer's output: ONE Philox4x32-10 call (key = seed, counter = (row,
-// layer << 24 | col / 32 * 4 + col / 2 % 4, step counter low, high word)) gives the 16 bits of the eight columns
-// {32 (col / 32) + 8 w + 2 (col / 2 % 4) + e : w < 4, e < 2}: word w, low half for e = 0, high half for e = 1.  These
-// are exactly the eight columns one lane of the epilogue holds in a row of a 32-column slice, so a lane draws once per
-// row and slice and the mask does not depend on the tile schedule, the CTA or the image that computes the column.
+// Dropout mask bits of row `row` of a layer's output (dropout_philox in dropout.cuh).
 // (Not inlined: inlined, the Philox rounds made ptxas spill 4-40 bytes in the gather roles of several instantiations at
 // the 80-register budget; as a call they use the caller's free registers and nothing spills.)
 __device__ __noinline__ uint4 dropout_bits(const SageParams& p, uint32_t row, uint32_t col) {
-  const ulonglong2 st = *reinterpret_cast<const ulonglong2*>(p.drop_state);
-  return Philox(st.x)(row, (p.drop_layer << 24) | ((col >> 5) << 2) | ((col >> 1) & 3u), (uint32_t)st.y, (uint32_t)(st.y >> 32));
+  return dropout_philox(p.drop_state, p.drop_layer, row, col);
 }
 
 __device__ __forceinline__ float dropout_apply(const SageParams& p, float x, uint32_t bits16) {

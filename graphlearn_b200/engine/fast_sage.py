@@ -38,8 +38,21 @@ gradient table and marks the rows read in a bitmap.  ``embed_lazy_adam`` then up
 (``torch.optim.SparseAdam``'s semantics at the dense Adam's step count), rewrites their E columns of the image and
 clears their gradient rows and bits, on a branch beside ``adam_pack``.
 
+Batch normalisation (``EgoGraphSAGE(batch_norm=True)``, one ``BatchNorm1d`` per hidden layer in ``model.norms``): every
+hop tensor (segment) of hidden layer l is ``H_l = dropout(relu(BN_l(Z_l)))``, normalised with its own batch mean and
+biased variance, and the running statistics are updated once per segment in hop order, as the reference's EgoGNN
+calls bn_func once per hop tensor.  The hidden layer's launch writes Z_l in fp32 (its conv has no bias, no ReLU, no
+dropout), and csrc/sage_bn.cu adds per BN layer:
+  forward   bn_colsum<false>  per-segment mean / rstd (shifted sums) + the module's running buffers, in place
+            bn_apply          H_l = dropout(relu(gamma x^ + beta)) in bf16, the epilogue's dropout mask
+  backward  sage_bwd_dz       sage_bwd_dw's dZ-only mode: dY_l, the routed gradient of the BN output, in bf16
+            bn_colsum<true>   per-segment sum(dY), sum(dY x^); d gamma, d beta into the flat gradient buffer
+            bn_bwd_apply      dZ_l in bf16, then dW_l on the dense dZ path (beside dA_l) and dA_l as without BN
+``infer_all`` / ``evaluate`` fold the eval-mode BN into inference-only weight images and bias; ``predict`` / ``embed``
+run the model's eval-mode autograd path.  Both use the running statistics.
+
 9 launches of this repo's kernels (0 library kernels) for the 2-layer flagship instead of ~60 on the autograd path
-(12 with the learned input embedding).
+(12 with the learned input embedding, 14 with batch normalisation).
 Layer l consumes hop pairs (i, i+1) for i in 0..L-l, exactly the EgoGNN
 recursion of graphlearn/python/nn/tf/model/ego_gnn.py:58-110.
 
@@ -63,6 +76,21 @@ from ..ops import sage as sage_ops
 from ..ops import sampling as S
 from ..parallel.runtime import Runtime, local_table_desc, native
 from ..store.shards import CsrShard, NodeTable
+
+
+@dataclass
+class HiddenBatchNorm:
+    """Batch normalisation of a hidden layer (``EgoGraphSAGE(batch_norm=True)``): the layer's launch writes Z (fp32, no
+    bias, no ReLU) and ``H = dropout(relu(BN(Z)))`` follows per segment with the segment's own batch statistics."""
+    norm: torch.nn.BatchNorm1d      # the model's module: gamma / beta (views of flat_p / flat_g) and the running buffers,
+                                    # which the forward statistics kernel updates in place
+    Z: torch.Tensor                 # fp32 [rows, out_dim], columns laid out as Hp's (N-split: image i at i * N)
+    mean: torch.Tensor              # fp32 [nseg, out_dim] batch mean of each segment
+    rstd: torch.Tensor              # fp32 [nseg, out_dim] 1 / sqrt(biased variance + eps)
+    gsum: torch.Tensor              # fp32 [nseg, 2, out_dim] backward: sum(dY), sum(dY x^) per segment
+    dY: torch.Tensor                # bf16 [rows, out_dim] gradient of the BN output (ReLU, dropout and routing applied)
+    tickets: torch.Tensor           # int32 [2, ceil(out_dim / 64)] zero between launches (forward / backward column sums)
+    drop: tuple                     # bn_fwd_apply's (drop_state, drop_p, drop_layer): dropout of H (p > 0), else off
 
 
 @dataclass
@@ -105,8 +133,10 @@ class SageLayer:
     argmax: Optional[torch.Tensor] = None
     amax: list = None
     # sage_bwd_dw's keyword arguments (seg_row0, seg_row1, self_src, nbr_src, seg_k, seg_scale, nbr_col0, dz_out,
-    # seg_self_scale, amax_src) for l < L, where dZ_l is computed from dA of the layer above
+    # seg_self_scale, amax_src) for l < L, where dZ_l is computed from dA of the layer above (with batch norm: dY, the
+    # gradient of the BN output, into bn.dY)
     bwd: Optional[dict] = None
+    bn: Optional[HiddenBatchNorm] = None
 
 
 @dataclass
@@ -147,6 +177,11 @@ class FastSageTrainer:
             raise ValueError("dropout must be in [0, 1), got %r" % (self.dropout,))
         if learn_input_embedding:
             self._check_input_embedding(rt, nodes, model, self.fanouts)
+        self.batch_norm = bool(getattr(model, "batch_norm", False))
+        if self.batch_norm and rt.world > 1:
+            raise ValueError("batch_norm trains on one GPU only (world = %d)" % rt.world)
+        if self.batch_norm and self.B < 2:
+            raise ValueError("batch_norm needs at least 2 rows per hop tensor (batch of %d roots)" % self.B)
         self.strategy = strategy
         self.C = native()
         dev = rt.device
@@ -210,9 +245,22 @@ class FastSageTrainer:
                 lo.bwd = dict(seg_row0=lo.offs[:-1], seg_row1=lo.offs[1:], self_src=da_seg + [None], nbr_src=[None] + da_seg,
                               seg_k=[1] + k_nbr, seg_scale=[1.0] + scale,
                               nbr_col0=sage_ops.padded_dims(c.in_self, c.in_nbr, c.agg_type)[0],
-                              dz_out=lo.dZ if lo.dA is not None else None, seg_self_scale=self_scale, amax_src=amax_src)
-            drop = (self.drop_state, self.dropout, l, offs[:-1]) if self.dropout > 0 and not last else (None, 0.0, 0, [])
-            outs = [Hp[offs[i]:offs[i + 1], :n_out] for i in range(nseg)]
+                              dz_out=lo.bn.dY if lo.bn is not None else lo.dZ if lo.dA is not None else None,
+                              seg_self_scale=self_scale, amax_src=amax_src)
+            bn = None
+            if self.batch_norm and not last:
+                # the launch writes Z; dropout moves to the BN apply kernel, which draws the epilogue's mask
+                Z = torch.zeros(rows, c.out_dim, dtype=torch.float32, device=dev)
+                bn = HiddenBatchNorm(
+                    norm=model.norms[l - 1], Z=Z,
+                    mean=torch.zeros(nseg, c.out_dim, dtype=torch.float32, device=dev), rstd=torch.zeros(nseg, c.out_dim, device=dev),
+                    gsum=torch.zeros(nseg, 2, c.out_dim, device=dev),
+                    dY=torch.zeros(rows, c.out_dim, dtype=torch.bfloat16, device=dev),
+                    tickets=torch.zeros(2, (c.out_dim + 63) // 64, dtype=torch.int32, device=dev),
+                    drop=(self.drop_state, self.dropout, l) if self.dropout > 0 else (None, 0.0, 0))
+            drop = (self.drop_state, self.dropout, l, offs[:-1]) if self.dropout > 0 and not last and bn is None \
+                else (None, 0.0, 0, [])
+            outs = [(Hp if bn is None else bn.Z)[offs[i]:offs[i + 1], :n_out] for i in range(nseg)]
             a_saves = [A[offs[i]:offs[i + 1]] for i in range(nseg)]
             self.layers.append(SageLayer(
                 conv=c, last=last, mode=sage_ops.MODE[c.agg_type], kt=kt, ns=ns, N=N, n_out=n_out,
@@ -223,7 +271,7 @@ class FastSageTrainer:
                 dW=c.weight_p.grad, db=c.bias.grad if c.bias is not None else None,
                 below=below, fwd=(self_base, nbr_base, self.n[:nseg], self.fanouts[:nseg], outs, a_saves),
                 drop=drop, da_alpha=1.0 / (1.0 - self.dropout) if l > 1 else 1.0,
-                argmax=argmax, amax=[] if argmax is None else [argmax[offs[i]:offs[i + 1]] for i in range(nseg)]))
+                argmax=argmax, amax=[] if argmax is None else [argmax[offs[i]:offs[i + 1]] for i in range(nseg)], bn=bn))
         self.emb: Optional[InputEmbedding] = None
         if learn_input_embedding:
             self.emb = self._make_input_embedding(lr if embedding_lr is None else float(embedding_lr))
@@ -462,6 +510,7 @@ class FastSageTrainer:
     # ------------------------------------------------------------------ what a subclass with other roots / loss replaces
     _fuse_ce = True         # the top layer's forward launch computes softmax-CE in its epilogue when it fits
     DROPOUT_SALT = 0x44524F50       # salt of the dropout seed ("DROP")
+    BN_BUFFERS = ("running_mean", "running_var", "num_batches_tracked")
 
     def _fill_slot(self, slot: int, seed_ids_host: torch.Tensor):
         """write one host batch into pinned staging slot `slot` (here: B seed vids)"""
@@ -529,8 +578,16 @@ class FastSageTrainer:
             else:                   # ... the contiguous row ranges of segments i / i + 1 of the layer below
                 d, self_ids, nbr_ids = ly.below, [None] * ly.nseg, [None] * ly.nseg
             ce = [self.nodes.labels.local, seeds, self.loss, ly.dZ, ly.db] if ly.fuse_ce else []
+            act = not ly.last and ly.bn is None         # ReLU + bf16 store in the epilogue; fp32 Z under batch norm
             C.sage_fused_multi(d, d, self_ids, nbr_ids, *ly.fwd, ly.mode, ly.img, ly.conv.bias, ly.N, ly.n_out,
-                               not ly.last, not ly.last, ce, self.rt.world, ly.ns, ly.amax, *ly.drop)
+                               act, act, ce, self.rt.world, ly.ns, ly.amax, *ly.drop)
+            b = ly.bn
+            if b is not None:
+                # per-segment statistics (+ the running buffers), then H = dropout(relu(BN(Z))) in bf16
+                m, n = b.norm, ly.conv.out_dim
+                C.bn_fwd_stats(b.Z, n, ly.offs, b.tickets[0], b.mean, b.rstd, m.running_mean, m.running_var,
+                               m.num_batches_tracked, m.eps, m.momentum)
+                C.bn_fwd_apply(b.Z, n, ly.offs, b.mean, b.rstd, m.weight, m.bias, ly.H, *b.drop)
             if ly.last and not ly.fuse_ce:
                 # wide / split top layer: the loss runs as its own kernel on the (padded) logits
                 self._top_loss(seeds)
@@ -546,10 +603,18 @@ class FastSageTrainer:
         #                 (the scales and the argmax routing of the layer above's aggregator are in ly.bwd)
         #   dA_l = dZ_l . W_l  (l >= 2) on sage_bwd_da (mma.sync) over the layer's forward weight images, times
         #                 1 / (1 - p) when H_{l-1} is dropped out (dZ_l itself stays unscaled: dW_l reads it too)
+        #   batch norm  : dY_l (routed as dZ_l above, into bn.dY) -> per-segment sum(dY), sum(dY x^) (+ d gamma, d beta)
+        #                 -> dZ_l = gamma rstd (dY - mean(dY) - x^ mean(dY x^)), then dW_l on the dense dZ path beside dA_l
         for ly in reversed(self.layers):
-            if ly.last:
+            b = ly.bn
+            if b is not None:
+                m, n = b.norm, ly.conv.out_dim
+                C.sage_bwd_dw(None, ly.H, a=None, dw=None, dbias=None, n_out=n, **ly.bwd)
+                C.bn_bwd_reduce(b.dY, b.Z, n, ly.offs, b.tickets[1], b.mean, b.rstd, b.gsum, m.weight.grad, m.bias.grad)
+                C.bn_bwd_apply(b.dY, b.Z, n, ly.offs, b.mean, b.rstd, m.weight, b.gsum, ly.dZ)
+            if ly.last or b is not None:
                 sA.wait_stream(main)
-                with torch.cuda.stream(sA):            # dW_L runs beside dA_L
+                with torch.cuda.stream(sA):            # dW_l runs beside dA_l
                     C.sage_bwd_dw(ly.dZ, None, [], [], [], [], [], [], 0, None, ly.A, ly.dW, None, ly.conv.out_dim)
             else:
                 C.sage_bwd_dw(None, ly.H, a=ly.A, dw=ly.dW, dbias=ly.db, n_out=ly.conv.out_dim, **ly.bwd)
@@ -718,7 +783,8 @@ class FastSageTrainer:
         a link trainer).  Layer l aggregates the FULL adjacency row of every node in ``self.csr`` (the neighbourhood
         training samples from) over the outputs of layer l - 1: one fused launch per layer, plus one hub pre-pass
         launch per layer when the CSR has rows above ``ops.sage.CSR_HUB_DEGREE``.  It uses the resident weight images
-        and the training forward's layer semantics (hidden layers ReLU -> bf16, top layer fp32), is deterministic and is
+        and the training forward's layer semantics (hidden layers ReLU -> bf16, top layer fp32; batch norm in eval mode, with
+        the running statistics, folded into the weights and bias), is deterministic and is
         the expectation that the sampled ``predict`` estimates.  Training state is not touched.  Collective when
         world > 1 (the hidden-layer tables are symmetric, allocated on the first call).  Export::
 
@@ -747,7 +813,15 @@ class FastSageTrainer:
                 out = res[:, :ly.n_out]
             else:
                 out = tabs[l][0].local[:, :ly.n_out]
-            plan.layer(desc, desc, vids, out, c.agg_type, ly.img, c.bias, ly.N, ly.n_out, not ly.last, not ly.last, ly.ns)
+            img, bias = ly.img, c.bias
+            if ly.bn is not None:
+                # eval-mode BN folded into the layer: s = gamma / sqrt(running_var + eps), W' = diag(s) W,
+                # b' = beta - s running_mean (inference-only images: ly.img belongs to the optimiser)
+                m = ly.bn.norm
+                s = m.weight / torch.sqrt(m.running_var + m.eps)
+                img = sage_ops.pack_images(c.weight_p * s[:, None], ly.N, ly.ns)
+                bias = (m.bias - s * m.running_mean).contiguous()
+            plan.layer(desc, desc, vids, out, c.agg_type, img, bias, ly.N, ly.n_out, not ly.last, not ly.last, ly.ns)
             if not ly.last:
                 desc = tabs[l][1]
                 rt.barrier()                                        # layer l + 1 reads peer rows of layer l
@@ -766,11 +840,16 @@ class FastSageTrainer:
               "steps": self._steps, "dropout_state": self.drop_state.cpu()}
         if self.emb is not None:
             sd["input_embedding"] = {"master": self.emb.master.clone(), "m": self.emb.m.clone(), "v": self.emb.v.clone()}
+        if self.batch_norm:
+            sd["batch_norm"] = [{k: getattr(ly.bn.norm, k).clone() for k in self.BN_BUFFERS} for ly in self.layers[:-1]]
         return sd
 
     def load_state_dict(self, sd):
         if self.emb is not None and "input_embedding" not in sd:
             raise ValueError("the checkpoint has no learned input embedding, which this trainer trains")
+        if self.batch_norm and len(sd.get("batch_norm", ())) != self.L - 1:
+            raise ValueError("the checkpoint has no batch-norm running statistics for the %d hidden layers this trainer "
+                             "normalises" % (self.L - 1))
         self.flat_p.copy_(sd["model"])
         self.repack()
         self.opt.load_state_dict(sd["opt"])
@@ -782,3 +861,7 @@ class FastSageTrainer:
             e, s = self.emb, sd["input_embedding"]
             e.master.copy_(s["master"]); e.m.copy_(s["m"]); e.v.copy_(s["v"])
             e.table.local[:, :e.master.size(1)] = e.master.to(torch.bfloat16)
+        if self.batch_norm:
+            for ly, st in zip(self.layers[:-1], sd["batch_norm"]):
+                for k in self.BN_BUFFERS:
+                    getattr(ly.bn.norm, k).copy_(st[k])
