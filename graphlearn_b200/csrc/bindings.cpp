@@ -38,10 +38,11 @@ void sage_fused_multi(const at::Tensor&, const at::Tensor&, const std::vector<c1
                       const c10::optional<at::Tensor>&, int64_t, int64_t, bool, bool,
                       const std::vector<c10::optional<at::Tensor>>&, int64_t, int64_t,
                       const std::vector<c10::optional<at::Tensor>>&, const c10::optional<at::Tensor>&, double, int64_t,
-                      const std::vector<int64_t>&);
+                      const std::vector<int64_t>&, int64_t, const std::vector<c10::optional<at::Tensor>>&);
 void sage_fused_csr(const at::Tensor&, const at::Tensor&, const at::Tensor&, const at::Tensor&, const at::Tensor&,
                     const std::vector<at::Tensor>&, const at::Tensor&, int64_t, const at::Tensor&,
-                    const c10::optional<at::Tensor>&, int64_t, int64_t, bool, bool, int64_t, int64_t);
+                    const c10::optional<at::Tensor>&, int64_t, int64_t, bool, bool, int64_t, int64_t, int64_t,
+                    const c10::optional<at::Tensor>&);
 int sm_count();
 void sage_set_debug_trace(const c10::optional<at::Tensor>&);
 // sage_bwd.cu
@@ -201,8 +202,13 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("a_saves"), py::arg("mode"), py::arg("w_img"), py::arg("bias"), py::arg("N"), py::arg("n_out"), py::arg("relu"),
         py::arg("out_bf16"), py::arg("ce"), py::arg("ce_world"), py::arg("n_imgs"),
         py::arg("amax") = std::vector<c10::optional<at::Tensor>>(), py::arg("drop_state") = py::none(), py::arg("drop_p") = 0.0,
-        py::arg("drop_layer") = 0, py::arg("drop_row0") = std::vector<int64_t>());
-  m.def("sage_fused_csr", &glb::sage_fused_csr);
+        py::arg("drop_layer") = 0, py::arg("drop_row0") = std::vector<int64_t>(), py::arg("split_half") = 0,
+        py::arg("partial") = std::vector<c10::optional<at::Tensor>>());
+  // (split_half / partial: one half of a split-K layer, see sage_fused.cu)
+  m.def("sage_fused_csr", &glb::sage_fused_csr, py::arg("tself_desc"), py::arg("tnbr_desc"), py::arg("self_vids"),
+        py::arg("csr_indptr"), py::arg("csr_indices"), py::arg("hubs"), py::arg("out"), py::arg("mode"), py::arg("w_img"),
+        py::arg("bias"), py::arg("N"), py::arg("n_out"), py::arg("relu"), py::arg("out_bf16"), py::arg("n_imgs"),
+        py::arg("plan_deg"), py::arg("split_half") = 0, py::arg("partial") = py::none());
   m.def("sm_count", &glb::sm_count);
   m.def("sage_set_debug_trace", &glb::sage_set_debug_trace);
   // (seg_self_scale / amax_src: the gradient routing of a gcn / max aggregation above, see sage_bwd.cu)

@@ -61,8 +61,10 @@ constexpr size_t kSmemLimit = 232448;
 
 enum SageMode : int { kConcatMean = 0, kConcatSum = 1, kGcnMean = 2, kConcatMax = 3 };
 // aggregation of an instantiation: kAggSum serves mean, sum and (sampled mode) gcn, whose scales are runtime factors;
-// kAggMax the max; kAggGcn the gcn mean of the CSR mode, which also loads the self row
-enum SageAgg : int { kAggSum = 0, kAggMax = 1, kAggGcn = 2 };
+// kAggMax the max; kAggGcn the gcn mean of the CSR mode, which also loads the self row.  kAggSplitK, or-ed into the
+// aggregation, marks the instantiations of the split-K launches (a layer whose padded K does not fit one CTA's shared
+// memory runs as a self half and a neighbour half, see sage_fused_multi): only they read the split-K fields of SageParams.
+enum SageAgg : int { kAggSum = 0, kAggMax = 1, kAggGcn = 2, kAggSplitK = 4 };
 
 struct SageSeg {
   const int64_t* self_vids;   // [M] or null (identity: self_base + m)
@@ -126,6 +128,14 @@ struct SageParams {
   uint32_t drop_thr;
   uint32_t drop_layer;
   int drop_row0[kMaxSegs];
+  // split-K launches only (AGG | kAggSplitK).  The layer's images hold both halves ((2 kp / 64) k-blocks each); w_img
+  // points at the first k-block of this launch's half in image 0 and w_img_stride (bytes) steps from image to image.
+  // a_save rows are the layer's full [self || agg] rows, a_ld elements apart.  The neighbour half adds part[s] (fp32, the
+  // self half's output, row stride part_ld, columns as the output's) to its accumulators before bias, ReLU and dropout.
+  long long w_img_stride;
+  int a_ld;
+  const float* part[kMaxSegs];
+  int part_ld;
 };
 
 // max aggregation: fold one neighbour chunk into the running column maxima
@@ -644,8 +654,12 @@ __global__ void __launch_bounds__(256) sage_hub_partial_kernel(const __grid_cons
 // DROP: the launch applies dropout (sampled mode only).  A template parameter rather than only the runtime field: with
 // the dropout path compiled into every instantiation (and the step counter advanced at p = 0 too) the headline step
 // measured 1.6 % slower at p = 0.
+// AGG | kAggSplitK: one half of a split-K layer (image stride, a_save row stride and, for the neighbour half, the self
+// half's fp32 partial added before the epilogue).
 template <int U, int DT, bool CSR, int AGG, bool DROP>
 __global__ void __launch_bounds__(kThreads, 1) sage_persist_kernel(const __grid_constant__ SageParams p) {
+  constexpr int kAgg = AGG & ~kAggSplitK;
+  constexpr bool kSplit = (AGG & kAggSplitK) != 0;
   if (p.dbg && threadIdx.x == 0) {
     unsigned long long gt; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt));
     p.dbg[(size_t)blockIdx.x * 64 + 60] = (long long)gt;
@@ -718,6 +732,23 @@ __global__ void __launch_bounds__(kThreads, 1) sage_persist_kernel(const __grid_
           __syncwarp();
           if (lane == 0) gmma::mbar_arrive(bars + kBarAFree + buf);
         }
+        if constexpr (kSplit) {                           // neighbour half: + the self half's x_self . W_self^T
+          const float* part = p.part[s];
+          if (part != nullptr) {
+            const int r0 = (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              if (r0 + 8 * h >= rows) continue;
+              const float* prow = part + (size_t)(m0 + r0 + 8 * h) * p.part_ld + img * p.N + sl * 32 + 2 * (lane & 3);
+#pragma unroll
+              for (int j = 0; j < 4; ++j) {
+                const float2 v = __ldcg(reinterpret_cast<const float2*>(prow + 8 * j));
+                d[4 * j + 2 * h] += v.x;
+                d[4 * j + 2 * h + 1] += v.y;
+              }
+            }
+          }
+        }
         // (warp < 4 here; the mask tells the compiler so: without it the <6, bf16> instantiation spills at 80 registers)
         if (sg.out) sage_epilogue_slice<DROP>(p, sg, sBias, d, m0, rows, sl * 32, warp & 3, lane, p.drop_row0[s] + m0, img * p.N);
       }
@@ -732,7 +763,8 @@ __global__ void __launch_bounds__(kThreads, 1) sage_persist_kernel(const __grid_
     // =================================================================== W image via TMA
     if (lane == 0) {
       gmma::mbar_arrive_expect_tx(bars + kBarW, (uint32_t)nkb * w_kb_bytes);
-      const uint8_t* src = reinterpret_cast<const uint8_t*>(p.w_img) + (size_t)img * nkb * w_kb_bytes;
+      const uint8_t* src = reinterpret_cast<const uint8_t*>(p.w_img) +
+                           (kSplit ? (size_t)img * (size_t)p.w_img_stride : (size_t)img * nkb * w_kb_bytes);
       for (int kb = 0; kb < nkb; ++kb)
         gmma::bulk_g2s(sW + (size_t)kb * w_kb_bytes, src + (size_t)kb * w_kb_bytes, w_kb_bytes, bars + kBarW);
     }
@@ -740,12 +772,12 @@ __global__ void __launch_bounds__(kThreads, 1) sage_persist_kernel(const __grid_
     gmma::mbar_wait(bars + kBarW, 0);
     GLB_DBG(1);
   } else if constexpr (CSR) {
-    sage_csr_gather<U, DT, AGG>(p, sA, a_buf_bytes, bars, sScr + (warp - kGatherWarp0) * kScrCap, tile_first, tile_stride,
-                           warp - kGatherWarp0, lane);
+    sage_csr_gather<U, DT, kAgg>(p, sA, a_buf_bytes, bars, sScr + (warp - kGatherWarp0) * kScrCap, tile_first, tile_stride,
+                                 warp - kGatherWarp0, lane);
   } else {
     // =================================================================== gather warps
     constexpr int VEC = Chunk<DT>::kVec;
-    constexpr bool kMax = AGG == kAggMax;
+    constexpr bool kMax = kAgg == kAggMax;
     const int gw = warp - kGatherWarp0;
     const int kp = p.kp_nbr > 0 ? p.kp_nbr : p.kp_self;
     const int d_self = p.tself.dim, d_nbr = p.tnbr.dim;
@@ -870,7 +902,7 @@ __global__ void __launch_bounds__(kThreads, 1) sage_persist_kernel(const __grid_
       uint8_t* sAt = sA + (size_t)(it & 1) * a_buf_bytes;
       if (row_ok) {
         const int m = cur.m0 + r;
-        __nv_bfloat16* a_row = (sg.a_save && img == 0) ? sg.a_save + (size_t)m * k_total : nullptr;
+        __nv_bfloat16* a_row = (sg.a_save && img == 0) ? sg.a_save + (size_t)m * (kSplit ? p.a_ld : k_total) : nullptr;
         if (has_self) put_chunk<VEC>(sAt, a_row, r, f0, sv);
         if (has_nbr) {
           float scale = 1.f;
@@ -1028,7 +1060,7 @@ static void launch_one(const SageParams& p, unsigned grid, size_t smem, cudaStre
 // row loads in flight per lane of the CSR mode (one instantiation per table dtype)
 constexpr int kCsrU = 5;
 
-static void launch_persist(SageParams& p, size_t smem, cudaStream_t stream, bool csr = false) {
+static void launch_persist(SageParams& p, size_t smem, cudaStream_t stream, bool csr = false, bool split = false) {
   if (p.total_tiles == 0) return;
   const unsigned grid = (unsigned)(p.n_imgs * std::min<int>(std::max(1, sm_count() / p.n_imgs), p.total_tiles));
   int kmax = 1;
@@ -1041,7 +1073,17 @@ static void launch_persist(SageParams& p, size_t smem, cudaStream_t stream, bool
                               else LAUNCH_DT3(6, false, AA, DD); } while (0)
   const int u = kmax <= 4 ? 4 : (kmax % 5 == 0 || kmax > 12) ? 5 : 6;
   const bool drop = p.drop_state != nullptr;
-  if (csr) {
+  constexpr int kSumS = kAggSum | kAggSplitK, kMaxS = kAggMax | kAggSplitK;
+  if (split && csr) {
+    if (p.mode == kConcatMax) LAUNCH_DT3(kCsrU, true, kMaxS, false);
+    else LAUNCH_DT3(kCsrU, true, kSumS, false);
+  } else if (split) {
+    // (U = 4 or 5 only: at U = 6 the max + dropout instantiations spill at 80 registers next to the partial's loads)
+#define LAUNCH_U45(AA, DD) do { if (u == 4) LAUNCH_DT3(4, false, AA, DD); else LAUNCH_DT3(5, false, AA, DD); } while (0)
+    if (p.mode == kConcatMax) { if (drop) LAUNCH_U45(kMaxS, true); else LAUNCH_U45(kMaxS, false); }
+    else if (drop) LAUNCH_U45(kSumS, true); else LAUNCH_U45(kSumS, false);
+#undef LAUNCH_U45
+  } else if (csr) {
     if (p.mode == kConcatMax) LAUNCH_DT3(kCsrU, true, kAggMax, false);
     else if (p.mode == kGcnMean) LAUNCH_DT3(kCsrU, true, kAggGcn, false);
     else LAUNCH_DT3(kCsrU, true, kAggSum, false);
@@ -1054,16 +1096,22 @@ static void launch_persist(SageParams& p, size_t smem, cudaStream_t stream, bool
 }
 
 // Launch-wide fields and checks shared by both entry points: tables, padded K, weight image, bias, output format.
-// Returns the dynamic shared memory of the launch; `b` keeps a contiguous copy of the bias alive.
+// split_half: 0 = the whole layer; 1 / 2 = the self / neighbour half of a split-K layer (a mean, sum or max layer
+// whose halves are padded alike), whose images hold both halves.  Returns the dynamic shared memory of the launch; `b`
+// keeps a contiguous copy of the bias alive.
 static size_t init_layer_params(SageParams& p, const at::Tensor& tself_desc, const at::Tensor& tnbr_desc, bool any_nbr, int64_t mode,
                                 const at::Tensor& w_img, const c10::optional<at::Tensor>& bias, at::Tensor& b, int64_t N,
-                                int64_t n_out, bool relu, bool out_bf16, int64_t n_imgs) {
+                                int64_t n_out, bool relu, bool out_bf16, int64_t n_imgs, int64_t split_half = 0) {
   std::memset(&p, 0, sizeof(p));
   p.tself = table_from_desc(tself_desc);
   p.tnbr = table_from_desc(tnbr_desc);
   p.mode = (int)mode;
-  p.kp_self = (mode == kGcnMean) ? 0 : pad_k(p.tself.dim);
-  p.kp_nbr = any_nbr ? pad_k(p.tnbr.dim) : 0;
+  TORCH_CHECK(split_half >= 0 && split_half <= 2, "split_half must be 0 (whole layer), 1 (self half) or 2 (neighbour half)");
+  if (split_half != 0)
+    TORCH_CHECK(mode != kGcnMean && pad_k(p.tself.dim) == pad_k(p.tnbr.dim),
+                "a split-K layer aggregates with mean, sum or max over equally padded self / neighbour inputs");
+  p.kp_self = (mode == kGcnMean || split_half == 2) ? 0 : pad_k(p.tself.dim);
+  p.kp_nbr = (any_nbr && split_half != 1) ? pad_k(p.tnbr.dim) : 0;
   if (mode == kGcnMean) TORCH_CHECK(p.tself.dim == p.tnbr.dim, "gcn mode needs equal dims");
   const int k_total = p.kp_self + p.kp_nbr;
   TORCH_CHECK(k_total >= 64, "empty layer");
@@ -1071,7 +1119,8 @@ static size_t init_layer_params(SageParams& p, const at::Tensor& tself_desc, con
   TORCH_CHECK(n_out <= N && n_out >= 1);
   TORCH_CHECK(n_imgs >= 1 && n_imgs <= 8 && (n_imgs == 1 || n_out == N), "bad image count");
   p.n_imgs = (int)n_imgs;
-  TORCH_CHECK(w_img.numel() == n_imgs * (int64_t)k_total * N, "weight image size mismatch: expected ", n_imgs * k_total * N, " got ", w_img.numel());
+  const int64_t k_layer = split_half != 0 ? 2 * (int64_t)k_total : k_total;      // K of the layer's images
+  TORCH_CHECK(w_img.numel() == n_imgs * k_layer * N, "weight image size mismatch: expected ", n_imgs * k_layer * N, " got ", w_img.numel());
   TORCH_CHECK((reinterpret_cast<uintptr_t>(w_img.data_ptr()) & 15) == 0, "weight image must be 16 B aligned");
   const size_t smem = (size_t)sage_smem_bytes(k_total, N);
   TORCH_CHECK(smem <= kSmemLimit, "tile does not fit in shared memory (", smem, " B); use the unfused path");
@@ -1086,6 +1135,10 @@ static size_t init_layer_params(SageParams& p, const at::Tensor& tself_desc, con
     p.bias_len = (int)b.numel();
   }
   p.w_img = w_img.data_ptr();
+  if (split_half != 0) {              // image i = (2 kp / 64) k-blocks of [N x 64]: the self half's, then the neighbour half's
+    p.w_img_stride = (long long)(k_layer / 64) * N * 128;
+    if (split_half == 2) p.w_img = reinterpret_cast<const char*>(w_img.data_ptr()) + (size_t)(k_total / 64) * N * 128;
+  }
   p.N = (int)N; p.n_out = (int)n_out; p.relu = relu ? 1 : 0; p.out_bf16 = out_bf16 ? 1 : 0;
   p.wshift_self = log2_or_neg(p.tself.world);
   p.wshift_nbr = log2_or_neg(p.tnbr.world);
@@ -1104,6 +1157,18 @@ static void set_seg_out(SageParams& p, SageSeg& sg, const at::Tensor& out, int64
   sg.out = reinterpret_cast<char*>(out.data_ptr());
 }
 
+// fp32 partial of segment s for the neighbour half of a split-K layer: the self half's output rows, whose columns are
+// laid out like the output's (image i at i * N)
+static void set_seg_part(SageParams& p, int s, const at::Tensor& t, int64_t M, int64_t n_out) {
+  TORCH_CHECK(t.is_cuda() && t.scalar_type() == at::kFloat && t.dim() == 2 && t.size(0) == M && t.size(1) == n_out &&
+              t.stride(1) == 1 && t.stride(0) >= (int64_t)p.n_imgs * p.N && t.stride(0) % 2 == 0 &&
+              (reinterpret_cast<uintptr_t>(t.data_ptr()) & 7) == 0,
+              "partial[i] must be an 8-byte aligned fp32 [M_i, n_out] view with an even row stride >= n_imgs * N");
+  TORCH_CHECK(p.part_ld == 0 || p.part_ld == t.stride(0), "all partial views must share the row stride");
+  p.part_ld = (int)t.stride(0);
+  p.part[s] = t.data_ptr<float>();
+}
+
 // Multi-segment entry point.  All segments share the tables, the weight image, the bias and the output
 // layout; segment i reads ids (self_vids[i], nbr_vids[i]) - or identity ids self_base[i] + m /
 // nbr_base[i] + m*k + j when the tensors are None - and writes outs[i] ([M_i, n_out]) and optionally
@@ -1115,6 +1180,11 @@ static void set_seg_out(SageParams& p, SageSeg& sg, const at::Tensor& out, int64
 // drop_p > 0: inverted dropout with rate drop_p after bias and ReLU (a hidden layer's training forward): the mask of
 // output element (drop_row0[i] + m, img * N + n) is a function of drop_state = {seed, step counter} (int64 [2], device),
 // drop_layer and that position only (see dropout_bits); drop_p = 0 (the default) launches exactly as before
+// split_half = 1 / 2: one half of a split-K layer, Z = x_self . W_self^T + agg . W_nbr^T, for a mean, sum or max layer
+// whose padded K = 2 kp does not fit one launch.  w_img is the layer's images (2 kp / 64 k-blocks each) and a_saves[i]
+// the [M_i, kp] views of the layer's [self || agg] rows that the half fills (row stride 2 kp).
+//   1 (self half): ks all 0, outs[i] = the fp32 partial (no bias, ReLU, dropout, amax or CE)
+//   2 (neighbour half): partial[i] = that partial, added to the accumulators before bias -> ReLU -> dropout -> store
 void sage_fused_multi(const at::Tensor& tself_desc, const at::Tensor& tnbr_desc,
                       const std::vector<c10::optional<at::Tensor>>& self_vids,
                       const std::vector<c10::optional<at::Tensor>>& nbr_vids,
@@ -1125,7 +1195,8 @@ void sage_fused_multi(const at::Tensor& tself_desc, const at::Tensor& tnbr_desc,
                       int64_t n_out, bool relu, bool out_bf16,
                       const std::vector<c10::optional<at::Tensor>>& ce, int64_t ce_world, int64_t n_imgs,
                       const std::vector<c10::optional<at::Tensor>>& amax, const c10::optional<at::Tensor>& drop_state,
-                      double drop_p, int64_t drop_layer, const std::vector<int64_t>& drop_row0) {
+                      double drop_p, int64_t drop_layer, const std::vector<int64_t>& drop_row0, int64_t split_half,
+                      const std::vector<c10::optional<at::Tensor>>& partial) {
   TORCH_CHECK(w_img.is_cuda() && w_img.scalar_type() == at::kBFloat16, "w_img must be CUDA bf16");
   TORCH_CHECK(mode >= kConcatMean && mode <= kConcatMax, "unknown aggregation mode ", mode);
   c10::cuda::CUDAGuard guard(w_img.device());
@@ -1137,8 +1208,15 @@ void sage_fused_multi(const at::Tensor& tself_desc, const at::Tensor& tnbr_desc,
   SageParams p;
   bool any_nbr = false;
   for (int s = 0; s < nseg; ++s) any_nbr = any_nbr || ks[s] > 0;
+  if (split_half == 1)
+    TORCH_CHECK(!any_nbr && ce.empty() && amax.empty() && drop_p == 0.0 && !relu && !out_bf16 && !(bias.has_value() && bias->defined()),
+                "the self half of a split-K layer reads no neighbours (ks = 0) and writes the bare fp32 partial");
+  if (split_half == 2) TORCH_CHECK(ce.empty(), "a split-K layer computes its loss outside the launch (no fused CE)");
+  TORCH_CHECK(split_half == 2 ? (int)partial.size() == nseg : partial.empty(),
+              "partial: one entry per segment of a neighbour-half launch, none otherwise");
   at::Tensor b;
-  const size_t smem = init_layer_params(p, tself_desc, tnbr_desc, any_nbr, mode, w_img, bias, b, N, n_out, relu, out_bf16, n_imgs);
+  const size_t smem = init_layer_params(p, tself_desc, tnbr_desc, any_nbr, mode, w_img, bias, b, N, n_out, relu, out_bf16, n_imgs,
+                                        split_half);
   p.nseg = nseg;
   {
     const int vec = p.tnbr.dtype == 0 ? 4 : 8;
@@ -1165,10 +1243,13 @@ void sage_fused_multi(const at::Tensor& tself_desc, const at::Tensor& tnbr_desc,
     set_seg_out(p, sg, outs[s], Ms[s], n_out, out_bf16);
     if (a_saves[s].has_value() && a_saves[s]->defined()) {
       const at::Tensor& a = *a_saves[s];
+      const int64_t a_ld = split_half != 0 ? 2 * (int64_t)k_total : k_total;     // split-K: the layer's full rows
       TORCH_CHECK(a.scalar_type() == at::kBFloat16 && a.dim() == 2 && a.size(0) == Ms[s] && a.size(1) == k_total &&
-                  a.stride(1) == 1 && a.stride(0) == k_total, "a_saves[i] must be a row-contiguous bf16 [M_i, K_total] view");
+                  a.stride(1) == 1 && a.stride(0) == a_ld, "a_saves[i] must be a bf16 [M_i, K_total] view with row stride ", a_ld);
       sg.a_save = reinterpret_cast<__nv_bfloat16*>(a.data_ptr());
+      p.a_ld = (int)a_ld;
     }
+    if (split_half == 2 && partial[s].has_value() && partial[s]->defined()) set_seg_part(p, s, *partial[s], Ms[s], n_out);
   }
   if (!amax.empty()) {
     TORCH_CHECK(mode == kConcatMax && (int)amax.size() == nseg, "amax needs a max launch and one entry per segment");
@@ -1232,7 +1313,7 @@ void sage_fused_multi(const at::Tensor& tself_desc, const at::Tensor& tnbr_desc,
   }
   p.dbg = g_dbg_ptr;
   plan_tiles(p);
-  launch_persist(p, smem, at::cuda::getCurrentCUDAStream());
+  launch_persist(p, smem, at::cuda::getCurrentCUDAStream(), false, split_half != 0);
 }
 
 // Layer-wise full-neighbourhood inference: ONE layer over every row of a CSR (row m of `out` aggregates the neighbour
@@ -1240,10 +1321,15 @@ void sage_fused_multi(const at::Tensor& tself_desc, const at::Tensor& tnbr_desc,
 // hubs = [] or [hub_map int32 [M] (-1 = ordinary row), hub_cptr int32 [n_hub + 1], chunks int64 [n_chunks, 2]
 // (edge ranges), part fp32 [>= n_chunks * kp_nbr]]: the hub rows' adjacency chunks are first summed into `part` by
 // sage_hub_partial_kernel.  plan_deg = mean degree of the ordinary rows (tile costing).
+// split_half = 2: the neighbour half of a split-K layer (see sage_fused_multi), which adds `partial` (fp32 [M, n_out],
+// the self half's output over the same rows) before the epilogue.
 void sage_fused_csr(const at::Tensor& tself_desc, const at::Tensor& tnbr_desc, const at::Tensor& self_vids,
                     const at::Tensor& csr_indptr, const at::Tensor& csr_indices, const std::vector<at::Tensor>& hubs,
                     const at::Tensor& out, int64_t mode, const at::Tensor& w_img, const c10::optional<at::Tensor>& bias,
-                    int64_t N, int64_t n_out, bool relu, bool out_bf16, int64_t n_imgs, int64_t plan_deg) {
+                    int64_t N, int64_t n_out, bool relu, bool out_bf16, int64_t n_imgs, int64_t plan_deg, int64_t split_half,
+                    const c10::optional<at::Tensor>& partial) {
+  TORCH_CHECK(split_half == 0 || split_half == 2, "the CSR mode runs a whole layer or the neighbour half of a split-K layer");
+  TORCH_CHECK((split_half == 2) == (partial.has_value() && partial->defined()), "the neighbour half needs the self half's partial");
   TORCH_CHECK(w_img.is_cuda() && w_img.scalar_type() == at::kBFloat16, "w_img must be CUDA bf16");
   c10::cuda::CUDAGuard guard(w_img.device());
   TORCH_CHECK(mode >= kConcatMean && mode <= kConcatMax, "unknown aggregation mode ", mode);
@@ -1256,7 +1342,8 @@ void sage_fused_csr(const at::Tensor& tself_desc, const at::Tensor& tnbr_desc, c
   TORCH_CHECK(M < (int64_t)INT32_MAX, "too many rows");
   SageParams p;
   at::Tensor b;
-  const size_t smem = init_layer_params(p, tself_desc, tnbr_desc, true, mode, w_img, bias, b, N, n_out, relu, out_bf16, n_imgs);
+  const size_t smem = init_layer_params(p, tself_desc, tnbr_desc, true, mode, w_img, bias, b, N, n_out, relu, out_bf16, n_imgs,
+                                        split_half);
   p.nseg = 1;
   SageSeg& sg = p.seg[0];
   sg.M = (int)M;
@@ -1265,6 +1352,7 @@ void sage_fused_csr(const at::Tensor& tself_desc, const at::Tensor& tnbr_desc, c
   p.out_stride = -1;
   set_seg_out(p, sg, out, M, n_out, out_bf16);
   TORCH_CHECK(sg.out != nullptr, "CSR mode needs an output");
+  if (split_half == 2) set_seg_part(p, 0, *partial, M, n_out);
   p.csr_indptr = csr_indptr.data_ptr<int64_t>();
   p.csr_indices = csr_indices.data_ptr<int64_t>();
   const cudaStream_t stream = at::cuda::getCurrentCUDAStream();
@@ -1304,7 +1392,7 @@ void sage_fused_csr(const at::Tensor& tself_desc, const at::Tensor& tnbr_desc, c
   }
   p.dbg = g_dbg_ptr;
   plan_tiles(p);
-  launch_persist(p, smem, stream, true);
+  launch_persist(p, smem, stream, true, split_half != 0);
 }
 
 // single-segment convenience wrapper (autograd op in ops/sage.py)
@@ -1327,7 +1415,7 @@ std::vector<at::Tensor> sage_fused_forward(const at::Tensor& tself_desc,
   if (M == 0) return {out, a_save};
   sage_fused_multi(tself_desc, tnbr_desc, {self_vids}, {nbr_vids}, {0}, {0}, {M}, {k}, {out},
                    {save_a ? c10::optional<at::Tensor>(a_save) : c10::nullopt}, mode, w_img, bias, N, n_out, relu, out_bf16,
-                   {}, 1, 1, {}, c10::nullopt, 0.0, 0, {});
+                   {}, 1, 1, {}, c10::nullopt, 0.0, 0, {}, 0, {});
   return {out, a_save};
 }
 
@@ -1346,7 +1434,7 @@ at::Tensor tc_linear_forward(const at::Tensor& a, const at::Tensor& w_img, const
   d[0] = 1; d[1] = K; d[2] = a.stride(0); d[3] = 1; d[4] = M; d[4 + kMaxWorld] = reinterpret_cast<int64_t>(a.data_ptr());
   at::Tensor desc = at::from_blob(d.data(), {(int64_t)d.size()}, at::kLong).clone();
   sage_fused_multi(desc, desc, {c10::nullopt}, {c10::nullopt}, {0}, {0}, {M}, {0}, {out}, {c10::nullopt}, kConcatMean, w_img, bias,
-                   N, n_out, relu, out_bf16, {}, 1, 1, {}, c10::nullopt, 0.0, 0, {});
+                   N, n_out, relu, out_bf16, {}, 1, 1, {}, c10::nullopt, 0.0, 0, {}, 0, {});
   return out;
 }
 

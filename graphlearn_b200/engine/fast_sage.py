@@ -51,8 +51,16 @@ dropout), and csrc/sage_bn.cu adds per BN layer:
 ``infer_all`` / ``evaluate`` fold the eval-mode BN into inference-only weight images and bias; ``predict`` / ``embed``
 run the model's eval-mode autograd path.  Both use the running statistics.
 
+Wide layers (``ops.sage.fused_layer_plan``): a mean, sum or max layer whose padded K = 2 kp (inputs 257-512 wide: K =
+1024) does not fit one CTA's shared memory runs split-K, as two launches of the same persistent kernel: the self half
+(no neighbours) writes x_self . W_self^T into an fp32 partial P and A[:, :kp], the neighbour half gathers and aggregates,
+fills A[:, kp:], adds P to its accumulators and runs the layer's epilogue (bias, ReLU, dropout, argmax bytes) exactly as
+one launch would.  The images are the layer's usual ones (each half is a k-block range of every image), so the backward
+and the fused Adam kernel see an ordinary layer with K = 2 kp.  A split top layer computes its loss with ``softmax_ce``.
+
 9 launches of this repo's kernels (0 library kernels) for the 2-layer flagship instead of ~60 on the autograd path
-(12 with the learned input embedding, 14 with batch normalisation).
+(12 with the learned input embedding, 14 with batch normalisation; one more per split-K layer, and one more when the
+top layer is split, for its loss kernel).
 Layer l consumes hop pairs (i, i+1) for i in 0..L-l, exactly the EgoGNN
 recursion of graphlearn/python/nn/tf/model/ego_gnn.py:58-110.
 
@@ -132,6 +140,12 @@ class SageLayer:
     # gradient routing; layer 1 has them only when it reads the learned input table (a feature table has no gradient)
     argmax: Optional[torch.Tensor] = None
     amax: list = None
+    # split-K forward (a mean / sum / max layer whose padded K = kt does not fit one launch): the self half writes
+    # x_self . W_self^T into P (fp32, columns as Hp's) and A[:, :kt / 2]; the neighbour half (`fwd`, `drop`, `amax`) fills
+    # A[:, kt / 2:], adds P and runs the epilogue.  fwd_self = the self half's (self_base, nbr_base, Ms, ks, outs, a_saves)
+    split: bool = False
+    P: Optional[torch.Tensor] = None
+    fwd_self: Optional[tuple] = None
     # sage_bwd_dw's keyword arguments (seg_row0, seg_row1, self_src, nbr_src, seg_k, seg_scale, nbr_col0, dz_out,
     # seg_self_scale, amax_src) for l < L, where dZ_l is computed from dA of the layer above (with batch norm: dY, the
     # gradient of the BN output, into bn.dY)
@@ -211,9 +225,8 @@ class FastSageTrainer:
             assert c.agg_type in ("mean", "sum", "max", "gcn"), "fast engine supports mean / sum / max / gcn aggregation"
             last = l == self.L
             kt = c.weight_p.size(1)
-            ns, N = sage_ops.split_images(kt, c.out_dim)
-            assert sage_ops.smem_fits(kt, N) and (ns == 1 or last or ns * N == c.out_dim), "layer does not fit the fused kernel"
-            assert sage_ops.fused_supported(c.in_self, c.in_nbr, min(c.out_dim, N), c.agg_type, max(self.fanouts))
+            halves, ns, N = sage_ops.fused_layer_plan(c.in_self, c.in_nbr, c.out_dim, c.agg_type, max(self.fanouts),
+                                                      last=last)
             n_out = c.out_dim if ns == 1 else N
             nseg = self.L - l + 1
             offs = [0]
@@ -262,16 +275,24 @@ class FastSageTrainer:
                 else (None, 0.0, 0, [])
             outs = [(Hp if bn is None else bn.Z)[offs[i]:offs[i + 1], :n_out] for i in range(nseg)]
             a_saves = [A[offs[i]:offs[i + 1]] for i in range(nseg)]
+            split, P, fwd_self = halves == 2, None, None
+            if split:
+                kp = kt // 2
+                P = torch.zeros(rows, ns * N, dtype=torch.float32, device=dev)
+                fwd_self = (self_base, nbr_base, self.n[:nseg], [0] * nseg, [P[offs[i]:offs[i + 1], :n_out] for i in range(nseg)],
+                            [a[:, :kp] for a in a_saves])
+                a_saves = [a[:, kp:] for a in a_saves]
             self.layers.append(SageLayer(
                 conv=c, last=last, mode=sage_ops.MODE[c.agg_type], kt=kt, ns=ns, N=N, n_out=n_out,
                 nseg=nseg, offs=offs, rows=rows,
-                fuse_ce=last and self._fuse_ce and ns == 1 and N <= 64,
+                fuse_ce=last and self._fuse_ce and ns == 1 and N <= 64 and not split,
                 Hp=Hp, H=Hp[:, :c.out_dim], A=A, dZp=dZp, dZ=dZp[:, :c.out_dim], dA=dA,
                 img=torch.zeros(kt * ns * N, dtype=torch.bfloat16, device=dev),
                 dW=c.weight_p.grad, db=c.bias.grad if c.bias is not None else None,
                 below=below, fwd=(self_base, nbr_base, self.n[:nseg], self.fanouts[:nseg], outs, a_saves),
                 drop=drop, da_alpha=1.0 / (1.0 - self.dropout) if l > 1 else 1.0,
-                argmax=argmax, amax=[] if argmax is None else [argmax[offs[i]:offs[i + 1]] for i in range(nseg)], bn=bn))
+                argmax=argmax, amax=[] if argmax is None else [argmax[offs[i]:offs[i + 1]] for i in range(nseg)], bn=bn,
+                split=split, P=P, fwd_self=fwd_self))
         self.emb: Optional[InputEmbedding] = None
         if learn_input_embedding:
             self.emb = self._make_input_embedding(lr if embedding_lr is None else float(embedding_lr))
@@ -579,8 +600,12 @@ class FastSageTrainer:
                 d, self_ids, nbr_ids = ly.below, [None] * ly.nseg, [None] * ly.nseg
             ce = [self.nodes.labels.local, seeds, self.loss, ly.dZ, ly.db] if ly.fuse_ce else []
             act = not ly.last and ly.bn is None         # ReLU + bf16 store in the epilogue; fp32 Z under batch norm
+            if ly.split:                                # split-K: the self half's partial first
+                C.sage_fused_multi(d, d, self_ids, [None] * ly.nseg, *ly.fwd_self, ly.mode, ly.img, None, ly.N, ly.n_out,
+                                   False, False, [], self.rt.world, ly.ns, split_half=1)
             C.sage_fused_multi(d, d, self_ids, nbr_ids, *ly.fwd, ly.mode, ly.img, ly.conv.bias, ly.N, ly.n_out,
-                               act, act, ce, self.rt.world, ly.ns, ly.amax, *ly.drop)
+                               act, act, ce, self.rt.world, ly.ns, ly.amax, *ly.drop,
+                               **({"split_half": 2, "partial": ly.fwd_self[4]} if ly.split else {}))
             b = ly.bn
             if b is not None:
                 # per-segment statistics (+ the running buffers), then H = dropout(relu(BN(Z))) in bf16
@@ -821,7 +846,8 @@ class FastSageTrainer:
                 s = m.weight / torch.sqrt(m.running_var + m.eps)
                 img = sage_ops.pack_images(c.weight_p * s[:, None], ly.N, ly.ns)
                 bias = (m.bias - s * m.running_mean).contiguous()
-            plan.layer(desc, desc, vids, out, c.agg_type, img, bias, ly.N, ly.n_out, not ly.last, not ly.last, ly.ns)
+            plan.layer(desc, desc, vids, out, c.agg_type, img, bias, ly.N, ly.n_out, not ly.last, not ly.last, ly.ns,
+                       split_k=ly.split)
             if not ly.last:
                 desc = tabs[l][1]
                 rt.barrier()                                        # layer l + 1 reads peer rows of layer l

@@ -51,12 +51,56 @@ def fused_supported(d_self: int, d_nbr: int, n_out: int, mode: str, k: int = 0, 
     if mode not in MODE or max(d_self, d_nbr) > 512 or n_out > 256:
         return False
     kp_self, kp_nbr = padded_dims(d_self, d_nbr, mode)
-    # a gather warp keeps the row pointers of one work item (1-4 destination rows) in a 64-entry scratch
-    lanes_row = max(kp_self, kp_nbr) // (4 if dtype == torch.float32 else 8)
-    rows_per_item = 32 // lanes_row if lanes_row < 32 else 1
-    if rows_per_item * (k + 1) > 64:
+    if k > max_fanout(max(kp_self, kp_nbr), dtype):
         return False
     return smem_fits(kp_self + kp_nbr, pad_n(n_out))
+
+
+def max_fanout(kp: int, dtype=torch.bfloat16) -> int:
+    """Largest fan-out the gather warps take for a half row padded to `kp`: a warp keeps the row pointers of one work
+    item (1-4 destination rows, k + 1 pointers each) in a 64-entry scratch."""
+    lanes_row = kp // (4 if dtype == torch.float32 else 8)
+    rows_per_item = 32 // lanes_row if lanes_row < 32 else 1
+    return 64 // rows_per_item - 1
+
+
+def fused_layer_plan(d_self: int, d_nbr: int, out_dim: int, mode: str, k: int = 0, dtype=torch.bfloat16,
+                     last: bool = False):
+    """How the fused trainers run a layer's forward: ``(halves, ns, N)``.  halves = 1 is one launch over the whole padded
+    K (``fused_supported``); halves = 2 is split-K, two launches of kp = K / 2 each (the self half, then the neighbour
+    half, which adds the self half's fp32 partial), for a mean, sum or max layer whose K = 2 kp does not fit one CTA's
+    shared memory.  ns images of N output columns each hold W (N-split); a hidden layer's ns * N must equal out_dim.
+    Raises ``ValueError`` naming the limit when neither fits."""
+    if mode not in MODE:
+        raise ValueError("unknown aggregation %r" % (mode,))
+    if max(d_self, d_nbr) > 512:
+        raise ValueError("the fused GraphSAGE layer takes inputs up to 512 wide (got %d and %d)" % (d_self, d_nbr))
+    kp_self, kp_nbr = padded_dims(d_self, d_nbr, mode)
+
+    def fits(kt):
+        ns, N = split_images(kt, out_dim)
+        return ns, N, smem_fits(kt, N) and (ns == 1 or last or ns * N == out_dim)
+
+    kt = kp_self + kp_nbr
+    ns, N, ok = fits(kt)
+    if ok and fused_supported(d_self, d_nbr, min(out_dim, N), mode, k, dtype):
+        return 1, ns, N
+    halves = 1
+    if not smem_fits(kt, N) and mode != "gcn" and kp_self == kp_nbr:
+        halves, kt = 2, kp_nbr
+        ns, N, ok = fits(kt)
+    what = "the fused GraphSAGE layer (%s, inputs %d + %d wide, %d outputs)" % (mode, d_self, d_nbr, out_dim)
+    if not smem_fits(kt, N):
+        raise ValueError("%s does not fit: a %d-column slice of W at K = %d exceeds the shared memory" % (what, N, kt))
+    if not ok:
+        raise ValueError("%s does not fit: hidden width %d does not split evenly over %d weight images of %d columns"
+                         % (what, out_dim, ns, N))
+    if k > max_fanout(max(kp_self, kp_nbr), dtype):
+        raise ValueError("%s: fan-out %d exceeds the limit of %d for inputs padded to %d columns"
+                         % (what, k, max_fanout(max(kp_self, kp_nbr), dtype), max(kp_self, kp_nbr)))
+    if halves == 1 or N > 256:
+        raise ValueError("%s does not fit: an image of %d output columns exceeds the kernel's 256" % (what, N))
+    return halves, ns, N
 
 
 def smem_bytes(k_total: int, n_pad: int) -> int:
@@ -135,17 +179,27 @@ class CsrPlan:
         self._part = {}                     # padded width -> fp32 partial rows of the hub chunks
 
     def layer(self, tself_desc, tnbr_desc, self_vids: torch.Tensor, out: torch.Tensor, mode: str, w_img: torch.Tensor,
-              bias: Optional[torch.Tensor], N: int, n_out: int, relu: bool, out_bf16: bool, n_imgs: int = 1):
+              bias: Optional[torch.Tensor], N: int, n_out: int, relu: bool, out_bf16: bool, n_imgs: int = 1,
+              split_k: bool = False):
         """One fused layer over every row: out[m] = act([x_self(self_vids[m]) || agg over the CSR row m] . W^T + b).
-        One launch, preceded by the hub pre-pass launch when the CSR has hubs."""
+        One launch, preceded by the hub pre-pass launch when the CSR has hubs.  ``split_k`` (a split-K layer, see
+        ``fused_layer_plan``): a sampled-mode launch with no neighbours first writes x_self . W_self^T into an fp32
+        partial, which the CSR launch over the neighbour half adds."""
+        C = native()
         hubs = []
         if self.hubs:
             kp = pad_k(int(tnbr_desc[1]))
             if kp not in self._part:
                 self._part[kp] = torch.empty(self.n_chunks * kp, dtype=torch.float32, device=self.indices.device)
             hubs = self.hubs + [self._part[kp]]
-        native().sage_fused_csr(tself_desc, tnbr_desc, self_vids, self.indptr, self.indices, hubs, out, MODE[mode], w_img,
-                                bias, N, n_out, relu, out_bf16, n_imgs, self.plan_deg)
+        part = None
+        if split_k:
+            M = self_vids.numel()
+            part = torch.empty(M, n_imgs * N, dtype=torch.float32, device=self.indices.device)[:, :n_out]
+            C.sage_fused_multi(tself_desc, tnbr_desc, [self_vids], [None], [0], [0], [M], [0], [part], [None], MODE[mode],
+                               w_img, None, N, n_out, False, False, [], 1, n_imgs, split_half=1)
+        C.sage_fused_csr(tself_desc, tnbr_desc, self_vids, self.indptr, self.indices, hubs, out, MODE[mode], w_img, bias, N,
+                         n_out, relu, out_bf16, n_imgs, self.plan_deg, 2 if split_k else 0, part)
 
 
 def logical_weight(weight_p: torch.Tensor, d_self: int, d_nbr: int, mode: str) -> torch.Tensor:
